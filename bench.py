@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py — augmented voxels/s of the 256^3 fp32 Compose pipeline on B200.
+"""bench.py — augmented voxels/s of the 256^3 fp32 Compose pipeline on H100.
 
     python bench.py --gpus N --steps K --warmup W            # our arm (CUDA kernels)
     python bench.py --impl reference --gpus N --steps K ...  # the reference's CPU path
+    python bench.py --steps K --dump-outputs DIR              # also save the last step's outputs
 
 A "step" is one pass of the hot path over one batch of synthetic volumes:
 ``Compose([Affine, ElasticDeformation, BiasField, Blur, Noise, Gamma])`` on
@@ -32,6 +33,8 @@ sys.path.insert(0, str(ROOT))
 
 VOL = 256
 ALGO_BYTES_PER_VOXEL_RESAMPLE = 8  # one fp32 read + one fp32 write (SURVEY.md §8d)
+HBM_GBS_DATASHEET = 3350.0  # H100 SXM data sheet (HBM3, 700 W card): the share-of-peak denominator
+DUMP_SAMPLES = 4 << 20  # values kept per image by --dump-outputs: 16 MiB of float32
 
 
 def parse_args():
@@ -54,7 +57,14 @@ def parse_args():
                     help="skip the configs[3] / configs[4] / gpu_baseline legs after the main timed region")
     ap.add_argument("--labels", action="store_true",
                     help="configs[3] shape: add an int16 LabelMap (nearest-neighbour resample) to every volume")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned as DIR/<image>.npy (float32; a fixed,"
+                         " seeded sample of at most DUMP_SAMPLES values per image)")
+    args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs saves what the CUDA path returned; --impl reference times a bounded CPU"
+                 " sample whose outputs are not comparable, so the two cannot be combined")
+    return args
 
 
 def pipeline_spec(workload):
@@ -79,6 +89,23 @@ def synth_volumes(batch, size, pin):
         g = torch.Generator().manual_seed(1000 + b)
         torch.rand((1, size, size, size), generator=g, out=out[b])
     return out
+
+
+def dump_outputs(batch, directory):
+    """Save what a caller of the timed path received: one float32 .npy per image.  Outputs
+    larger than DUMP_SAMPLES values keep the same seeded, sorted positions on every run, so
+    two builds given the same arguments can be compared value for value."""
+    import numpy as np
+
+    out_dir = Path(directory)
+    out_dir.mkdir(parents=True, exist_ok=True)
+    for name, ib in batch.images.items():
+        flat = ib.data.reshape(-1)
+        if flat.numel() > DUMP_SAMPLES:
+            g = torch.Generator().manual_seed(20240917)
+            idx = torch.randint(flat.numel(), (DUMP_SAMPLES,), generator=g).sort().values
+            flat = flat[idx.to(flat.device)]
+        np.save(out_dir / f"{name}.npy", flat.to(torch.float32).cpu().numpy())
 
 
 # ----------------------------------------------------------------------------
@@ -238,6 +265,8 @@ def run_b200(args, rank, world, local_rank):
     wall_end = time.perf_counter()
     ms = t0.elapsed_time(t1)
     launches = ops.launches() - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(out, args.dump_outputs)
     clocks = sampler.stop(wall_begin, wall_end) if sampler else None
     k1_ms = [s.elapsed_time(e) for s, e in k1_events]
     del out
@@ -270,7 +299,7 @@ def run_b200(args, rank, world, local_rank):
         # in flight, so the copy-in of step n+1 overlaps the copy-out of step n; (b) the plain
         # call `pipeline(batch)`, step by step, reported beside it.
         # Warm-up: the loop keeps three pinned 2 GiB result buffers alive (in flight, yielded, held
-        # by the consumer) and page-locking one takes ~0.6 s; device slices are cached by torch's
+        # by the consumer) and page-locking one is slow; device slices are cached by torch's
         # allocators too.  Warm up until a round of steps allocates nothing new.
         torch.manual_seed(4321 + rank)
         for _ in range(6):
@@ -346,7 +375,7 @@ def run_b200(args, rank, world, local_rank):
     peaks_path = ROOT / "MEASURED_PEAKS.json"
     if peaks_path.exists():
         peaks = json.loads(peaks_path.read_text())
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", HBM_GBS_DATASHEET))
     k1_avg_ms = sum(k1_ms) / len(k1_ms) if k1_ms else float("nan")
     achieved = ALGO_BYTES_PER_VOXEL_RESAMPLE * voxels / (k1_avg_ms * 1e-3) / 1e9
     value = world * voxels * args.steps / (ms * 1e-3)
@@ -373,7 +402,7 @@ def run_b200(args, rank, world, local_rank):
             "global_batch": world * args.batch,
             "parallelism": f"dp{world} (independent volumes, no data-path collective)",
             "noise_normals": args.noise,
-            "l2_policy": "inputs (%.1f GiB/GPU) larger than L2 (126 MB)" % (voxels * 4 / 2**30),
+            "l2_policy": "inputs (%.1f GiB/GPU) larger than L2 (50 MB)" % (voxels * 4 / 2**30),
             "includes": "host param sampling + table upload + all kernels of the step",
         },
         "gpu_launches": launches,
@@ -385,12 +414,10 @@ def run_b200(args, rank, world, local_rank):
             "peak": peak,
             "unit": "GB/s",
             "frac": achieved / peak,
-            "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "fallback 6650 GB/s",
+            "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "H100 SXM data sheet, 3350 GB/s",
             "algorithmic_bytes_per_launch": ALGO_BYTES_PER_VOXEL_RESAMPLE * voxels,
             "avg_launch_ms": k1_avg_ms,
             "share_of_step": sum(k1_ms) / ms if k1_ms else None,
-            "traffic": k1_traffic(args),
-            "traffic_source": "profiles/r2_k1_traffic.json (committed ncu --set full capture, not this run)",
         },
         "clocks": clocks,
     }
@@ -483,7 +510,7 @@ def extra_legs(args, dev, pipeline_spec, tio, ops):
         ms = t0.elapsed_time(t1) / steps
         lab = [s.elapsed_time(e) for s, e in label_ms]
         lab_avg = sum(lab) / len(lab)
-        peak = 6576.4
+        peak = HBM_GBS_DATASHEET
         peaks_path = ROOT / "MEASURED_PEAKS.json"
         if peaks_path.exists():
             peak = float(json.loads(peaks_path.read_text()).get("hbm_gbs", peak))
@@ -508,7 +535,7 @@ def extra_legs(args, dev, pipeline_spec, tio, ops):
         out["config4"] = queue_unet_leg(args, dev, tio)
     except Exception as exc:  # never lose the headline line to an extra
         out["config4"] = {"error": repr(exc)}
-    # ---- the reference's op sequence on CUDA tensors (the existing Blackwell path) ----
+    # ---- the reference's op sequence on CUDA tensors (what TorchIO runs on the same GPU) ----
     if not args.no_cpu_baseline:
         try:
             out["gpu_baseline"] = gpu_reference(args, dev)
@@ -576,7 +603,7 @@ def queue_unet_leg(args, dev, tio):
 
 def gpu_reference(args, dev):
     """The reference's op sequence (oracle/torch_port.py = what TorchIO runs) on CUDA tensors of
-    the same B200: the existing Blackwell path the fused kernels are compared with."""
+    the same GPU: the existing CUDA path the fused kernels are compared with."""
     import numpy as np
 
     import torchio_b200 as tio
@@ -617,7 +644,7 @@ def gpu_reference(args, dev):
         "unit": "voxels/s",
         "kind": "port-on-cuda",
         "sample": f"median of 3 steps of batch {b} x 1x{size}^3 fp32, same Compose, torch {torch.__version__}"
-                  " CUDA ops (ATen sm_100 kernels) on the same GPU, inputs resident, host randn + H2D as the reference does",
+                  " CUDA ops (ATen kernels) on the same GPU, inputs resident, host randn + H2D as the reference does",
         "seconds_per_step": times[1],
         "spread_s": [times[0], times[-1]],
     }
@@ -629,16 +656,6 @@ def gpu_reference(args, dev):
 # ----------------------------------------------------------------------------
 
 
-def k1_traffic(args):
-    """DRAM bytes per K1 launch (dram__bytes_read.sum + dram__bytes_write.sum, mean of the affine and
-    the elastic launch) from the committed `ncu --set full` capture of this workload
-    (profiles/r2_k1_traffic.json) — not re-measured in this run — or None when the run differs."""
-    path = ROOT / "profiles" / "r2_k1_traffic.json"
-    if not path.exists() or args.batch != 32 or args.size != VOL:
-        return None
-    return json.loads(path.read_text()).get("bytes_per_launch")
-
-
 def cpu_reference(args, steps, warmup):
     import numpy as np
 
@@ -647,8 +664,8 @@ def cpu_reference(args, steps, warmup):
 
     cores = os.cpu_count() or 1
     torch.set_num_threads(cores)
-    # bounded sample: ~13 s per step at batch 2 on the GPU box's 128 host threads; one volume per
-    # step for long runs keeps the whole --steps run within a few minutes
+    # bounded sample: a batch-2 step takes 14-16 s on the 16 host threads of an H100 80GB HBM3
+    # machine; one volume per step for long runs keeps the whole --steps run within a few minutes
     b = args.cpu_sample_batch if steps * args.cpu_sample_batch <= 12 else 1
     size = args.size
     with warnings.catch_warnings():

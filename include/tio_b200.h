@@ -1,5 +1,5 @@
 /*
- * tio_b200.h — C-ABI of the B200-native 3-D augmentation hot path.
+ * tio_b200.h — C-ABI of the CUDA-native (sm_90a) 3-D augmentation hot path.
  *
  * Drop-in boundary for the TorchIO v2 (2.0.0a2 @ 2b019d2) transform kernels.
  * The reference has no FFI layer: its seam is the Python method

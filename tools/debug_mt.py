@@ -1,4 +1,4 @@
-import sys; sys.path.insert(0, '/root/repo')
+import sys; sys.path.insert(0, __import__('os').path.dirname(__import__('os').path.dirname(__import__('os').path.abspath(__file__))))
 import torch
 from torchio_b200 import ops
 for seed, offset, n in [(0, 0, 16), (1234, 0, 64), (1234, 0, 4096), (7, 0, 3 * 2**20 + 1600), (99, 40 * 2**20, 2**21 + 32)]:

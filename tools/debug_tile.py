@@ -1,5 +1,5 @@
 import sys, numpy as np, torch
-sys.path.insert(0, '/root/repo')
+sys.path.insert(0, __import__('os').path.dirname(__import__('os').path.dirname(__import__('os').path.abspath(__file__))))
 from torchio_b200 import ops
 torch.manual_seed(0)
 x = torch.rand(1, 1, 64, 64, 64, device='cuda')

@@ -1,5 +1,5 @@
 """cProfile of the host thread while host-resident batches stream through the device
-(where do the ~3 ms of host time per slice go?).  GPU box: python tools/e2e_profile.py"""
+(where does the host time per slice go?).  On a GPU machine: python tools/e2e_profile.py"""
 import cProfile
 import os
 import pstats

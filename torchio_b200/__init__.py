@@ -1,10 +1,10 @@
-"""torchio_b200 — B200-native 3-D augmentation hot path behind the TorchIO v2 API.
+"""torchio_b200 — CUDA-native 3-D augmentation hot path behind the TorchIO v2 API.
 
 Drop-in for the reference's spatial + intensity augmentation chain
 (`Affine`, `ElasticDeformation`, `Spatial`, `BiasField`, `Blur`, `Noise`,
 `Gamma`, `Compose`) and its patch path (`UniformSampler`, `Queue`,
 `SubjectsLoader`) on tensor-backed `Subject` / `SubjectsBatch` data.  The
-tensor math runs in hand-written sm_100a CUDA kernels exposed through the C-ABI
+tensor math runs in hand-written sm_90a (H100) CUDA kernels exposed through the C-ABI
 of ``include/tio_b200.h``; see DESIGN.md and INTEGRATION.md.
 """
 

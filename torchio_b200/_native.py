@@ -1,7 +1,7 @@
 """ctypes binding of the C-ABI library (include/tio_b200.h).
 
 The library is built in-tree by ``__graft_entry__.build()`` /
-``torchio_b200/csrc/build.py`` (nvcc, sm_100a) and loaded from
+``torchio_b200/csrc/build.py`` (nvcc, sm_90a) and loaded from
 ``torchio_b200/csrc/libtio_b200.so``.  There is no fallback: if the library is
 missing or a call fails, a RuntimeError carrying ``tio_last_error()`` is raised.
 """

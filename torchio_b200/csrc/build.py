@@ -1,10 +1,10 @@
-"""Build libtio_b200.so in-tree with nvcc for sm_100a (no JIT cache, no torch headers).
+"""Build libtio_b200.so in-tree with nvcc for sm_90a (no JIT cache, no torch headers).
 
     python torchio_b200/csrc/build.py [--force] [--verbose]
 
 The shared library exports exactly the C-ABI of include/tio_b200.h and is
 loaded with ctypes by torchio_b200/_native.py.  nvcc cross-compiles without a
-GPU; the .so travels to the GPU box with the repo snapshot.
+GPU.
 """
 
 from __future__ import annotations
@@ -20,12 +20,14 @@ ROOT = HERE.parent.parent
 SOURCES = ["error.cu", "resample.cu", "resample_tile.cu", "resample_fast.cu", "intensity.cu", "fused_intensity.cu",
            "mt19937_jump.cpp", "mt19937.cu", "patches.cu", "stats.cu", "labels.cu"]
 HEADERS = [HERE / "common.cuh", HERE / "intensity_common.cuh", HERE / "resample_common.cuh", HERE / "resample_tile.cuh", HERE / "tma.cuh",
-           ROOT / "include" / "tio_b200.h"]
+           ROOT / "include" / "tio_b200.h",
+           Path(__file__).resolve()]  # the flags below: objects built for another architecture are rebuilt
 OBJ = HERE / "_obj"
 OUT = HERE / "libtio_b200.so"
 
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    *ARCH,
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "-Xptxas", "-v",
@@ -68,7 +70,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     if failed:
         raise RuntimeError(f"nvcc failed for {failed}")
     objects = [str(OBJ / (Path(s).stem + ".o")) for s in SOURCES]
-    proc = subprocess.run(["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", str(OUT),
+    proc = subprocess.run(["nvcc", *ARCH, "-shared", "-o", str(OUT),
                            *objects], capture_output=True, text=True)
     if proc.returncode != 0:
         sys.stderr.write(proc.stdout + proc.stderr)

@@ -1,4 +1,4 @@
-// common.cuh — shared helpers for the sm_100a kernels behind include/tio_b200.h
+// common.cuh — shared helpers for the sm_90a kernels behind include/tio_b200.h
 #pragma once
 
 #include <cuda_runtime.h>
@@ -38,7 +38,9 @@ void set_error(const char* fmt, ...);
     }                                                                        \
   } while (0)
 
-constexpr int kNumSMs = 148;  // B200
+// SM count of the current device (132 on an H100 SXM, 114 on an H100 PCIe), read once per
+// device: the grid caps scale with it
+int num_sms();
 
 // ---- align_corners=True linear-upsample index/weights (ATen semantics) -----
 // scale = (n_in-1)/(n_out-1) in fp32 (precomputed on the host with the same

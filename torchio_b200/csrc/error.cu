@@ -12,6 +12,19 @@ void set_error(const char* fmt, ...) {
   vsnprintf(g_error, sizeof(g_error), fmt, ap);
   va_end(ap);
 }
+
+int num_sms() {
+  constexpr int kMaxDevices = 64;
+  static int cache[kMaxDevices] = {};  // 0 = not read yet; racing first reads store the same value
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) dev = -1;
+  int n = dev >= 0 ? __atomic_load_n(&cache[dev], __ATOMIC_RELAXED) : 0;
+  if (n > 0) return n;
+  if (dev < 0 || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
+    return 132;  // the launch that follows reports the device error
+  __atomic_store_n(&cache[dev], n, __ATOMIC_RELAXED);
+  return n;
+}
 }  // namespace tio
 
 extern "C" const char* tio_last_error(void) { return tio::g_error; }

@@ -723,8 +723,8 @@ march6_kernel(const float* __restrict__ src, float* __restrict__ dst, int B, int
 
   // Input planes arrive through a per-thread cp.async FIFO (M6_PF slots of 16 bytes in shared
   // memory, no registers): M6_PF-1 loads are in flight per thread while a plane is processed.
-  // Without it the unrolled phases issue one dependent load at a time (8 KB in flight per SM
-  // against the ~35 KB that 6.5 TB/s x DRAM latency needs).  Planes are consumed strictly in
+  // Without it the unrolled phases issue one dependent load at a time (8 KB in flight per SM,
+  // far less than HBM bandwidth x DRAM latency needs to keep the memory system busy).  Planes are consumed strictly in
   // order; slot = plane mod M6_PF; the slot of plane i-1 is refilled while plane i is consumed.
   float4* fifo = reinterpret_cast<float4*>(g + ((ns + 3) / 4) * 4) + tid;  // [M6_PF][256]
   auto fifo_issue = [&](int pl) {

@@ -214,7 +214,7 @@ gamma_kernel(const float* __restrict__ src, float* __restrict__ dst, int64_t per
 
 static inline int ew_blocks(int64_t nvec) {
   int64_t blocks = (nvec + 255) / 256;
-  int64_t cap = (int64_t)kNumSMs * 16;
+  int64_t cap = (int64_t)num_sms() * 16;
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
   return (int)blocks;

@@ -65,7 +65,7 @@ template <typename T>
 static void launch_onehot(const void* src, int B, int64_t vox, const void* labels, int n, float* dst,
                           cudaStream_t st) {
   int64_t blocks = (vox / 4 + 255) / 256;
-  if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
+  if (blocks > num_sms() * 16) blocks = num_sms() * 16;
   if (blocks < 1) blocks = 1;
   onehot_kernel<T><<<dim3((unsigned)blocks, B), 256, 0, st>>>(
       (const T*)src, vox, (const typename LabelTable<T>::type*)labels, n, dst);
@@ -75,7 +75,7 @@ template <typename T>
 static void launch_argmax(const float* sampled, int B, int n, int64_t vox, const void* labels, float pad,
                           void* dst, cudaStream_t st) {
   int64_t blocks = (vox + 255) / 256;
-  if (blocks > kNumSMs * 16) blocks = kNumSMs * 16;
+  if (blocks > num_sms() * 16) blocks = num_sms() * 16;
   if (blocks < 1) blocks = 1;
   label_argmax_kernel<T><<<dim3((unsigned)blocks, B), 256, 0, st>>>(
       sampled, n, vox, (const typename LabelTable<T>::type*)labels, pad, (T*)dst);

@@ -228,7 +228,7 @@ extern "C" int tio_min_sample0(const float* src, int C, int64_t n, float* fill, 
   const bool vec = (((uintptr_t)src & 15) == 0) && ((n & 3) == 0);
   int64_t work = vec ? (n >> 2) : n;
   int blocks = (int)((work + 255) / 256);
-  if (blocks > kNumSMs * 8) blocks = kNumSMs * 8;
+  if (blocks > num_sms() * 8) blocks = num_sms() * 8;
   if (blocks < 1) blocks = 1;
   if (vec)
     min_kernel<true><<<dim3(blocks, C), 256, 0, st>>>(src, n, fill);

@@ -1,9 +1,7 @@
 // resample_fast.cu — K1 for fp32 images, trilinear: TMA-staged tiles with one-fma coordinates.
 //
-// What the profile of the exact kernel (resample_tile.cu) says at the bench size
-// (profiles/r1_ncu_full_k1_final_batch32.csv): 65 warp-instructions per voxel-warp, 27 of
-// them the reference's fp32 rounding chain (sgemm order, normalise / un-normalise round
-// trip) and 23 per-tile set-up; the shared-memory data pipe is 70 % busy, issue 57 %.
+// A large share of the exact kernel's (resample_tile.cu) instructions per voxel is the
+// reference's fp32 rounding chain (sgemm order, normalise / un-normalise round trip).
 //
 // For a voxel whose 8 taps all lie inside the volume that chain only reproduces the
 // reference's own coordinate noise (<= 1.5e-5 voxel): no fill decision and no zero halo
@@ -106,9 +104,8 @@ __device__ __noinline__ void slow_tile(const ResampleArgs& a, const TileArgs& ta
 // they were read from.  Along the walk the sampling point advances by about one voxel in I and
 // by little in J/K, so for most voxels the lower-plane taps ARE the previous voxel's upper-plane
 // taps: they stay in registers and the four lower-plane loads run predicated, only for the lanes
-// whose cell moved in J/K or skipped a plane.  ncu (profiles/r2_ncu_full_k1_fast_batch32.csv): the
-// kernel sits at 82 % of the shared-memory data pipe with 2.1 wavefronts per LDS (rotated rows
-// step across box rows); a predicated load touches ~20 % of the lanes and takes ~1.3.
+// whose cell moved in J/K or skipped a plane: the kernel is bound by the shared-memory data
+// pipe (rotated rows step across box rows, so an LDS takes about two wavefronts).
 struct Carry {
   float u00, u01, u10, u11;
   uint32_t up;  // address of the (i + 1, j, k) tap the values came from; 0xffffffff = none
@@ -240,11 +237,10 @@ resample_fast_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_cons
     mbar_expect_tx(bar, (uint32_t)((small ? NBOXS : NBOX) * 4));
     tma_load_4d(box_u32, small ? &tmap_s : &tmap, rec.z, rec.y, rec.x, b * a.C, bar);
   }
-  // The CTA that will run ~one resident wave later finds its box in L2: ncu shows 31 % of the
-  // affine kernel's warp time at the barrier behind the TMA load, most of it the HBM latency of
-  // the quarter of the box no neighbouring tile has touched yet.
-  // Elastic launches only: affine launches gain nothing (1.399 vs 1.388 ms) and the prefetch takes
-  // their L2 throughput from 53 % to 87 % of peak.
+  // The CTA that will run ~one resident wave later finds its box in L2 instead of waiting at the
+  // barrier behind its TMA load for the HBM latency of the part of the box no neighbouring tile
+  // has touched yet.  Elastic launches only, and only when TIO_B200_K1_PREFETCH sets a distance
+  // (off by default, see launch_resample_tile).
   if (HAS_CP && ta.prefetch_ahead && tid == 224) {
     const unsigned ahead = tile_id + ta.prefetch_ahead;
     if (ahead < gridDim.x * gridDim.y * gridDim.z) {

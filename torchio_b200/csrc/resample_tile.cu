@@ -273,8 +273,8 @@ __device__ __forceinline__ void walk_column(
     const f2 u1 = mul2(add2(add2(norm_div2<FASTDIV>(q1, hd1, rc1), mone2), one2), bc(hs1));
     const f2 u2 = mul2(add2(add2(norm_div2<FASTDIV>(q2, hd2, rc2), mone2), one2), bc(hs2));
     if (MODE == TIO_NEAREST) {
-      // scalar adds: ptxas contracts mul.rn.f32x2 + add.rn.f32x2 into one FFMA2 (seen in SASS),
-      // which rounds exact ties (u = n + 0.5) down instead of to even
+      // round-to-nearest-even adds on the unpacked lanes: a multiply fused into this add
+      // would round exact ties (u = n + 0.5) down instead of to even
       float u0a, u0b, u1a, u1b, u2a, u2b;
       unpack2(u0, u0a, u0b); unpack2(u1, u1a, u1b); unpack2(u2, u2a, u2b);
       const float r0a = __fadd_rn(u0a, kMagic), r0b = __fadd_rn(u0b, kMagic);
@@ -564,7 +564,7 @@ static bool fastdiv_admitted(float d, cudaStream_t st) {
   unsigned long long* bad = nullptr;
   if (cudaMalloc(&bad, 8) == cudaSuccess) {
     cudaMemsetAsync(bad, 0, 8, st);
-    verify_fastdiv_kernel<<<kNumSMs * 16, 256, 0, st>>>(d, (float)(1.0 / (double)d), bad);
+    verify_fastdiv_kernel<<<num_sms() * 16, 256, 0, st>>>(d, (float)(1.0 / (double)d), bad);
     unsigned long long host = 1;
     if (cudaMemcpyAsync(&host, bad, 8, cudaMemcpyDeviceToHost, st) == cudaSuccess &&
         cudaStreamSynchronize(st) == cudaSuccess)
@@ -693,10 +693,12 @@ int launch_resample_tile(const ResampleArgs& a, int dtype, int mode, bool exact_
   ta.sp_in_one = (a.sp_in[0] == 1.f && a.sp_in[1] == 1.f && a.sp_in[2] == 1.f);
   ta.sp_out_one = (a.sp_out[0] == 1.f && a.sp_out[1] == 1.f && a.sp_out[2] == 1.f);
   ta.magic_bytes = (unsigned)kMagicBits << 2;
-  {  // TIO_B200_K1_PREFETCH: tiles of look-ahead of the L2 box prefetch (development knob; 0 = off)
+  {  // TIO_B200_K1_PREFETCH: tiles of look-ahead of the L2 box prefetch (development knob).  Off by
+     // default: on an H100 SXM at 400 W every distance tried (99, 198, 396 tiles) made the K1
+     // launches slower than none (2.93-3.00 vs 2.70 ms per 32 x 256^3 launch, affine + elastic mean).
     static const int ahead = []() {
       const char* e = getenv("TIO_B200_K1_PREFETCH");
-      return e ? atoi(e) : 222;  // half a resident wave (148 SMs x 3 CTAs): 1.706 -> 1.630 ms elastic, 1.399 -> 1.388 affine
+      return e ? atoi(e) : 0;
     }();
     ta.prefetch_ahead = ahead > 0 ? (unsigned)ahead : 0u;
   }

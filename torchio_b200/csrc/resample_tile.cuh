@@ -1,6 +1,6 @@
 // resample_tile.cuh — pieces shared by the two K1 tile kernels (resample_tile.cu: exact
 // coordinate chain, label maps; resample_fast.cu: relaxed one-fma coordinates for fp32 images):
-// tile geometry, the per-tile bounds pre-pass, shared-memory loads, packed fp32x2 arithmetic.
+// tile geometry, the per-tile bounds pre-pass, shared-memory loads, two-lane fp32 arithmetic.
 #pragma once
 #include <cuda.h>
 
@@ -129,7 +129,7 @@ tile_bounds_kernel(const ResampleArgs a, const int box, const int kalign, const 
                    const int bk_s, int4* __restrict__ records) {
   // ONE THREAD per tile: the work of a tile is a short serial chain (index arithmetic, a dozen
   // table loads, interval arithmetic); a warp per tile left 31 lanes idle and made the pass
-  // latency-bound at 14 waves of warps per SM (0.055 / 0.155 ms per 32 x 256^3 launch).
+  // latency-bound (many waves of one-lane warps per SM).
   const int tiles_i = (a.OI + XT - 1) / XT, tiles_j = (a.OJ + XT - 1) / XT, tiles_k = (a.OK + XT - 1) / XT;
   const int64_t n_tiles = (int64_t)a.B * tiles_i * tiles_j * tiles_k;
   const int64_t tile = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -229,7 +229,7 @@ struct LiEntry {  // per output plane of the tile: I-axis lerp of the control gr
   int off0, off1;  // i0 * plane, i1 * plane (floats)
   float l0, l1;
 };
-struct __align__(16) LiPair {  // planes (2p, 2p+1) of the tile, weights laid out as fp32x2 operands
+struct __align__(16) LiPair {  // planes (2p, 2p+1) of the tile, weights laid out as two-lane operands
   int off0, off1;    // of plane 2p
   float l0a, l0b;    // l0 of plane 2p, 2p+1
   float l1a, l1b;
@@ -237,46 +237,26 @@ struct __align__(16) LiPair {  // planes (2p, 2p+1) of the tile, weights laid ou
   int pad;
 };
 
-// ---- packed fp32x2 arithmetic (sm_100 FFMA2/FADD2/FMUL2) ---------------------------
-// Two IEEE fp32 lanes per 64-bit register, each rounded exactly like the scalar
-// instruction; a scalar operand packed with itself is encoded by ptxas as a broadcast
-// (no extra register).  The walk is issue-bound, so halving the FP instruction count
-// by treating two output planes at once is the lever (the FP32 pipe does the same work).
-typedef unsigned long long f2;
-__device__ __forceinline__ f2 pack2(float lo, float hi) {
-  f2 r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ f2 bc(float x) { return pack2(x, x); }
+// ---- two-lane fp32 arithmetic ----------------------------------------------------
+// Two output planes are walked at once, lane by lane.  sm_90 has no packed fp32x2
+// instructions, so each lane is one scalar instruction with an explicit rounding mode
+// (the __f*_rn intrinsics are never contracted), rounded exactly like the one-plane path.
+struct f2 {
+  float lo, hi;
+};
+__device__ __forceinline__ f2 pack2(float lo, float hi) { return f2{lo, hi}; }
+__device__ __forceinline__ f2 bc(float x) { return f2{x, x}; }
 __device__ __forceinline__ void unpack2(f2 v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
+  lo = v.lo;
+  hi = v.hi;
 }
 __device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) {
-  f2 d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  return f2{__fmaf_rn(a.lo, b.lo, c.lo), __fmaf_rn(a.hi, b.hi, c.hi)};
 }
-__device__ __forceinline__ f2 add2(f2 a, f2 b) {
-  f2 d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ f2 sub2(f2 a, f2 b) {
-  f2 d;
-  asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ f2 mul2(f2 a, f2 b) {
-  f2 d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ f2 add2_rd(f2 a, f2 b) {
-  f2 d;
-  asm("add.rm.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
+__device__ __forceinline__ f2 add2(f2 a, f2 b) { return f2{__fadd_rn(a.lo, b.lo), __fadd_rn(a.hi, b.hi)}; }
+__device__ __forceinline__ f2 sub2(f2 a, f2 b) { return f2{__fsub_rn(a.lo, b.lo), __fsub_rn(a.hi, b.hi)}; }
+__device__ __forceinline__ f2 mul2(f2 a, f2 b) { return f2{__fmul_rn(a.lo, b.lo), __fmul_rn(a.hi, b.hi)}; }
+__device__ __forceinline__ f2 add2_rd(f2 a, f2 b) { return f2{__fadd_rd(a.lo, b.lo), __fadd_rd(a.hi, b.hi)}; }
 // affine_row (resample_common.cuh) on two positions at once
 __device__ __forceinline__ f2 affine_row2(const float* m, f2 pi, f2 pj, f2 pk) {
   f2 acc = mul2(pi, bc(m[0]));

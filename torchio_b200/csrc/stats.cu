@@ -212,7 +212,7 @@ extern "C" int tio_moments(const float* src, const uint8_t* mask, int64_t n, dou
   cudaStream_t st = (cudaStream_t)stream;
   TIO_CHECK_CUDA(cudaMemsetAsync(out3, 0, 3 * sizeof(double), st));
   int blocks = (int)((n / 4 + 255) / 256);
-  if (blocks > kNumSMs * 8) blocks = kNumSMs * 8;
+  if (blocks > num_sms() * 8) blocks = num_sms() * 8;
   if (blocks < 1) blocks = 1;
   moments_kernel<<<blocks, 256, 0, st>>>(src, mask, n, out3);
   TIO_CHECK_LAUNCH();
@@ -239,7 +239,7 @@ extern "C" int tio_quantiles(const float* src, const uint8_t* mask, int64_t n, c
   const double q0 = q_host[0], q1 = m > 1 ? q_host[1] : 0.0;
   select_init_kernel<<<1, 1, 0, st>>>(state, m);
   int blocks = (int)((n + 255) / 256);
-  if (blocks > kNumSMs * 8) blocks = kNumSMs * 8;
+  if (blocks > num_sms() * 8) blocks = num_sms() * 8;
   const size_t hbytes = (size_t)kTargets * 2048 * sizeof(unsigned);
   TIO_CHECK_CUDA(cudaMemsetAsync(hist, 0, hbytes, st));
   select_hist_kernel<0><<<blocks, 256, 0, st>>>(src, mask, n, state, hist);
@@ -264,7 +264,7 @@ extern "C" int tio_rescale(const float* src, float* dst, int B, int64_t per_elem
   const bool vec = ((per_elem & 3) == 0) && (((uintptr_t)src | (uintptr_t)dst) & 15) == 0;
   const int64_t work = vec ? per_elem / 4 : per_elem;
   int bx = (int)((work + 255) / 256);
-  const int cap = (kNumSMs * 16 + B - 1) / B;
+  const int cap = (num_sms() * 16 + B - 1) / B;
   if (bx > cap) bx = cap < 1 ? 1 : cap;
   TIO_CHECK_ARG(B <= 65535, "tio_rescale: batch too large");
   dim3 grid(bx, B);

@@ -1,5 +1,5 @@
 // tma.cuh — tensor-map encoding (driver entry point, no -lcuda) and the PTX
-// wrappers for mbarrier + cp.async.bulk.tensor used by the sm_100a kernels.
+// wrappers for mbarrier + cp.async.bulk.tensor used by the sm_90a kernels.
 #pragma once
 
 #include <cuda.h>

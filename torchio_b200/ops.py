@@ -63,8 +63,8 @@ class _StagingRing:
     Allocating pinned memory per call (``torch.empty(pin_memory=True)``) looked
     free but is not: while the host runs ahead of the GPU the caching host
     allocator cannot recycle blocks whose copies are still queued, so every call
-    ends in ``cudaHostAlloc`` — measured at ~1.2 ms of GPU stall per upload on
-    B200.  The ring allocates once; a slot is reused only after the event
+    ends in ``cudaHostAlloc``, which stalls the GPU.  The ring allocates once; a
+    slot is reused only after the event
     recorded behind its last copy has completed."""
 
     SLOTS = 64
@@ -127,8 +127,8 @@ def upload(device: torch.device, *arrays):
     else:
         stage = torch.empty(offset, dtype=torch.uint8, pin_memory=torch.cuda.is_available())
     # plain memcpy through numpy views: torch's CPU copy_ fans tensors above 32 KiB out to
-    # the intra-op thread pool, and waking 100+ OpenMP threads on a busy host was measured
-    # to stall this call for tens of milliseconds (tools/host_stalls3.py)
+    # the intra-op thread pool, and waking a large OpenMP pool on a busy host stalls this
+    # call (tools/host_stalls3.py finds such stalls)
     stage_np = stage.numpy()
     for s in specs:
         if s is None:
