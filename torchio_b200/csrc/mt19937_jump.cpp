@@ -2,8 +2,8 @@
 //
 // The reference draws its noise with torch.randn on a CPU mt19937 generator
 // (transforms/intensity/noise.py:166-178), one sequential stream per call.  To
-// replay that stream on the GPU the stream is cut into segments of L = 2^20
-// words whose start states are obtained by jump-ahead (Haramoto, Matsumoto,
+// replay that stream on the GPU the stream is cut into segments of L = 2^21
+// words (mt19937_layout.h) whose start states are obtained by jump-ahead (Haramoto, Matsumoto,
 // Nishimura, Panneton, L'Ecuyer 2008): with F the one-word state transition and
 // phi its characteristic polynomial, F^J = g_J(F), g_J = x^J mod phi.  This file
 // computes phi (Berlekamp-Massey on 2*19937 output bits) and the polynomials
@@ -17,6 +17,7 @@
 #include <vector>
 
 #include "../../include/tio_b200.h"
+#include "mt19937_layout.h"
 
 namespace {
 
@@ -142,17 +143,19 @@ static bool build_field(Field& f) {
 
 }  // namespace
 
-// ---- table layout -------------------------------------------------------------
+// ---- table layout (mt19937_layout.h) ---------------------------------------------
 //   uint32 header[8] = {magic, log2(L), S2, S1, n_polys, stride_u16, 0, 0}
 //   per polynomial (n_polys = (S2-1) + (S1-1)), `stride_u16` uint16 entries:
 //       [count_lo, count_hi, idx0, idx1, ...]   (set-bit positions, ascending)
 //   fine polynomials h_1..h_{S2-1} first, then coarse b_1..b_{S1-1}.
-static constexpr uint32_t kMagic = 0x4d544a31u;  // "MTJ1"
-static constexpr int kLog2L = 20, kS2 = 32, kS1 = 64;
-static constexpr int kStride = 10496;  // >= 2 + max popcount observed (~10.1k), multiple of 64
+using tio_mt::kLog2L;
+using tio_mt::kMagic;
+using tio_mt::kS1;
+using tio_mt::kS2;
+using tio_mt::kStride;
 
 extern "C" size_t tio_mt19937_table_bytes(void) {
-  return 32 + (size_t)((kS2 - 1) + (kS1 - 1)) * kStride * sizeof(uint16_t);
+  return tio_mt::kHeaderBytes + (size_t)tio_mt::kPolys * kStride * sizeof(uint16_t);
 }
 
 extern "C" int tio_mt19937_build_table(void* blob, size_t bytes) {
@@ -161,8 +164,8 @@ extern "C" int tio_mt19937_build_table(void* blob, size_t bytes) {
   if (!build_field(f)) return 2;
   uint32_t* header = (uint32_t*)blob;
   header[0] = kMagic; header[1] = kLog2L; header[2] = kS2; header[3] = kS1;
-  header[4] = (kS2 - 1) + (kS1 - 1); header[5] = kStride; header[6] = header[7] = 0;
-  uint16_t* out = (uint16_t*)((char*)blob + 32);
+  header[4] = tio_mt::kPolys; header[5] = kStride; header[6] = header[7] = 0;
+  uint16_t* out = (uint16_t*)((char*)blob + tio_mt::kHeaderBytes);
   auto emit = [&](const Bits& p, int slot) -> bool {
     uint16_t* dst = out + (size_t)slot * kStride;
     uint32_t count = 0;
@@ -199,7 +202,7 @@ extern "C" int tio_mt19937_apply_poly_host(const void* blob, int slot, const uin
                                            uint32_t* out) {
   const uint32_t* header = (const uint32_t*)blob;
   if (header[0] != kMagic || slot < 0 || slot >= (int)header[4]) return 1;
-  const uint16_t* p = (const uint16_t*)((const char*)blob + 32) + (size_t)slot * header[5];
+  const uint16_t* p = (const uint16_t*)((const char*)blob + tio_mt::kHeaderBytes) + (size_t)slot * header[5];
   const uint32_t count = p[0] | ((uint32_t)p[1] << 16);
   std::vector<uint32_t> seq(kDeg + 624 + 8);
   memcpy(seq.data(), in, 624 * 4);

@@ -529,11 +529,15 @@ _mt_host_table: Tensor | None = None
 _mt_device_tables: dict = {}
 _mt_lock = threading.Lock()
 MT_MAX_WORDS = 1 << 31  # stream positions the two-level jump table reaches
+# uint32 header of the table the library builds (csrc/mt19937_layout.h): magic "MTJ1",
+# log2(segment length), S2, S1, polynomials, stride.  Tables for another segment length
+# have the same size, so a cached file is only used when its header matches.
+MT_TABLE_HEADER = (0x4D544A31, 21, 16, 64, 78, 10496)
 
 
 def mt19937_host_table() -> Tensor:
     """Jump-ahead table (constants of MT19937): loaded from the file written at
-    build time, else computed on the host (~2 s) and cached."""
+    build time if its size and header match, else computed on the host (~2 s) and cached."""
     global _mt_host_table
     with _mt_lock:
         if _mt_host_table is None:
@@ -541,7 +545,9 @@ def mt19937_host_table() -> Tensor:
             nbytes = lib.tio_mt19937_table_bytes()
             blob = None
             if _MT_TABLE_FILE.exists() and _MT_TABLE_FILE.stat().st_size == nbytes:
-                blob = torch.from_numpy(np.fromfile(_MT_TABLE_FILE, dtype=np.uint8))
+                cached = np.fromfile(_MT_TABLE_FILE, dtype=np.uint8)
+                if tuple(int(v) for v in cached[:24].view(np.uint32)) == MT_TABLE_HEADER:
+                    blob = torch.from_numpy(cached)
             if blob is None:
                 blob = torch.zeros(nbytes, dtype=torch.uint8)
                 _native.call("tio_mt19937_build_table", blob.data_ptr(), nbytes)
