@@ -30,7 +30,7 @@
 extern "C" {
 #endif
 
-#define TIO_ABI_VERSION 1
+#define TIO_ABI_VERSION 2
 
 /* element types accepted by tio_resample (images: F32; label maps: the rest) */
 enum tio_dtype {
@@ -168,19 +168,6 @@ int tio_upload(const void* host_pinned, void* dst_device, size_t bytes, void* st
 int tio_min_sample0(const float* src, int C, int64_t n, float* fill, void* stream);
 
 /*
- * K2 — bias field: dst = src * exp(trilerp_align_corners(coarse)) (or / for
- * the inverse).  Replaces _apply_bias_per_element / _generate_bias_field
- * (transforms/intensity/bias_field.py:201-255, 296-341).
- *   coarse    [B][C][si][sj][sk] fp32, drawn on the host by torch.normal from
- *             the recorded seeds (bias_field.py:281-293,316-329)
- *   identity  [B] bytes, non-zero = copy the row exactly (std == 0), or NULL
- * In-place (src == dst) allowed.
- */
-int tio_bias_field(const float* src, float* dst, int B, int C, int I, int J, int K,
-                   const float* coarse, int si, int sj, int sk,
-                   const uint8_t* identity, int divide, void* stream);
-
-/*
  * K3 — separable Gaussian blur with replicate (clamp) addressing, axes I, J,
  * K in that order.  Replaces _gaussian_smooth{,_shared,_per_element}
  * (transforms/intensity/blur.py:129-252) = 3 x (F.pad replicate + F.conv3d).
@@ -223,37 +210,6 @@ int tio_randn_mt19937(uint64_t seed, uint64_t offset, uint64_t n, float* z,
                       void* stream);
 
 /*
- * K4 — additive Gaussian / Rician noise.  Replaces _sample_noise + add +
- * _restore_gated_out (transforms/intensity/noise.py:98-178).
- *   dst = src + (mean[b] + std[b] * z)                       (Gaussian)
- *   dst = sqrt((src + n1)^2 + n2^2), n_i = mean + std * z_i  (Rician)
- *   z, z2    standard normals, same shape as src (z2 NULL unless Rician); the
- *            reference draws them with torch.randn on a CPU mt19937 generator
- *   keep     [B] bytes or NULL; rows with keep == 0 are copied exactly
- * In-place allowed.
- */
-int tio_noise(const float* src, float* dst, int B, int64_t per_elem,
-              const float* mean, const float* std, const uint8_t* keep,
-              const float* z, const float* z2, void* stream);
-
-/*
- * K4b — same, with normals generated in registers from Philox4x32-7 keyed by
- * (seed, global element index): statistically equivalent, NOT the reference
- * stream.  `rician` selects the two-draw variant.
- */
-int tio_noise_philox(const float* src, float* dst, int B, int64_t per_elem,
-                     const float* mean, const float* std, const uint8_t* keep,
-                     uint64_t seed, int rician, void* stream);
-
-/*
- * K5 — gamma: dst = sign(src) * |src| ^ gamma[b].  Replaces
- * data.sign() * data.abs().pow(gamma)  (transforms/intensity/gamma.py:88-90).
- * In-place allowed.
- */
-int tio_gamma(const float* src, float* dst, int B, int64_t per_elem,
-              const float* gamma, void* stream);
-
-/*
  * Data-derived parameters of Standardize / Normalize, computed where the batch lives
  * (the reference reads batch element 0 on the host: standardize.py:52-79, normalize.py:121-139,
  * 332-366, _statistics.py:11-45).
@@ -281,16 +237,30 @@ int tio_rescale(const float* src, float* dst, int B, int64_t per_elem, float lo,
                 const uint8_t* keep, int flags, void* stream);
 
 /*
- * Fused intensity chain: what Compose([BiasField, Blur, Noise, Gamma]) computes,
- * in two HBM passes.  Any stage may be absent (NULL table / noise_mode 0):
- *   v   = src * exp(trilerp(coarse))   (/ when bias_divide)  if coarse != NULL
- *   v   = blur_I(blur_J(blur_K(v)))                          if taps   != NULL
- *   v   = v + mean[b] + std[b] * n  (or Rician)               if noise_mode != 0
- *   dst = sign(v) |v|^gamma[b]                                if gamma  != NULL
- * Equal to running K2, K3, K4, K5 one after another up to fp32 summation order
- * (the separable passes commute; the reference order is I, J, K).
- *   noise_mode 1: normals supplied in z (z2 for the second Rician draw)
- *   noise_mode 2: Philox4x32-7 keyed by philox_seed (NOT the reference stream)
+ * Intensity chain: what Compose([BiasField, Blur, Noise, Gamma]) computes, in
+ * at most two HBM passes.  Each stage is absent when its table is NULL (noise:
+ * noise_mode 0), and an absent stage leaves v unchanged:
+ *   K2  v   = src * exp(trilerp(coarse))   (/ when bias_divide)  if coarse != NULL
+ *   K3  v   = blur_I(blur_J(blur_K(v)))                          if taps   != NULL
+ *   K4  v   = v + (mean[b] + std[b] * n)   (or Rician)           if noise_mode != 0
+ *   K5  dst = sign(v) |v|^gamma[b]                                if gamma  != NULL
+ * A single transform runs as a call with only its own stage set.  The blur
+ * passes commute up to fp32 summation order (the reference order is I, J, K).
+ *   K2  replaces _apply_bias_per_element / _generate_bias_field
+ *       (transforms/intensity/bias_field.py:201-255, 296-341); coarse is
+ *       [B][C][si][sj][sk] fp32, drawn on the host by torch.normal from the
+ *       recorded seeds (bias_field.py:281-293, 316-329)
+ *   K3  see tio_blur for taps / radius / R / axes_mask
+ *   K4  replaces _sample_noise + add + _restore_gated_out
+ *       (transforms/intensity/noise.py:98-178); Rician:
+ *       sqrt((v + n1)^2 + n2^2), n_i = mean + std * z_i
+ *       noise_mode 1: standard normals supplied in z (z2 for the second Rician
+ *                     draw), same shape as src; tio_randn_mt19937 replays the
+ *                     reference's torch.randn(generator=CPU) stream
+ *       noise_mode 2: Philox4x32-7 normals generated in registers, keyed by
+ *                     philox_seed: statistically equivalent, NOT the reference stream
+ *   K5  replaces data.sign() * data.abs().pow(gamma)
+ *       (transforms/intensity/gamma.py:88-90)
  *   per-element identity rows (bias_identity[b], all radii 0, keep[b] == 0,
  *   gamma[b] == 1) pass through every stage as bit-exact copies
  *   scratch: B*C*I*J*K floats, required when axes_mask has bit 1 or 2 (J/K)

@@ -27,7 +27,7 @@ def test_library_exports_every_declared_symbol():
 
 def test_abi_version_and_error_string():
     lib = _native.lib()
-    assert lib.tio_abi_version() == 1
+    assert lib.tio_abi_version() == 2
     assert isinstance(lib.tio_last_error(), bytes)
 
 
@@ -35,7 +35,8 @@ def test_bad_arguments_fail_loudly_without_touching_the_gpu():
     import pytest
 
     with pytest.raises(RuntimeError, match="null"):
-        _native.call("tio_gamma", None, None, 1, 16, None, None)
+        _native.call("tio_intensity_fused", None, None, None, 1, 1, 1, 1, 16, None, 0, 0, 0, None, 0,
+                     None, None, 0, 0, None, None, None, None, None, 0, 0, 0, None, None)
     with pytest.raises(RuntimeError, match="alias"):
         buf = ctypes.create_string_buffer(64)
         p = ctypes.addressof(buf)

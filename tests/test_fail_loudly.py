@@ -86,7 +86,7 @@ def test_ops_raise_on_host_tensors():
 
     x = torch.rand((1, 1, 8, 8, 8))
     with pytest.raises((RuntimeError, ValueError, TypeError)):
-        ops.gamma(x, torch.ones(1))
+        ops.intensity_fused(x, gamma=torch.ones(1))
     with pytest.raises((RuntimeError, ValueError, TypeError)):
         ops.crop_patches(x[0], [[0, 0, 0]], (4, 4, 4))
     lab = (x * 4).to(torch.int16)

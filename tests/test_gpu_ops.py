@@ -137,6 +137,7 @@ def test_min_sample0():
 
 
 def test_intensity_kernels_vs_c_oracle():
+    """Each intensity stage on its own: a tio_intensity_fused call with only that stage set."""
     from torchio_b200 import ops
 
     c_port = _orc()
@@ -153,7 +154,8 @@ def test_intensity_kernels_vs_c_oracle():
         for divide in (0, 1):
             want = torch.empty_like(x)
             lib.orc_bias_field(p(x), p(want), b, c, *shape[2:], p(coarse), 4, 5, 6, p(ident), divide)
-            got = ops.bias_field(x.cuda(), coarse.cuda(), ident.cuda(), divide=bool(divide)).cpu()
+            got = ops.intensity_fused(x.cuda(), coarse=coarse.cuda(), bias_identity=ident.cuda(),
+                                      bias_divide=bool(divide)).cpu()
             assert (got - want).abs().max() <= 2e-6 * float(want.abs().max())
             assert torch.equal(got[1], x[1])
         # blur
@@ -175,32 +177,38 @@ def test_intensity_kernels_vs_c_oracle():
         for zz in (None, z2):
             want = torch.empty_like(x)
             lib.orc_noise(p(x), p(want), b, ctypes.c_int64(n), p(mean), p(std), p(keep), p(z), p(zz))
-            got = ops.noise(x.cuda(), mean.cuda(), std.cuda(), keep.cuda(), z.cuda(),
-                            None if zz is None else zz.cuda()).cpu()
+            got = ops.intensity_fused(x.cuda(), mean=mean.cuda(), std=std.cuda(), keep=keep.cuda(),
+                                      z=z.cuda(), z2=None if zz is None else zz.cuda(), noise_mode=1,
+                                      rician=zz is not None).cpu()
             assert (got - want).abs().max() <= 1e-6
             assert torch.equal(got[1], x[1])
         # gamma
         gam = torch.tensor([0.8, 1.0, 1.3][:b])
         want = torch.empty_like(x)
         lib.orc_gamma(p(x), p(want), b, ctypes.c_int64(n), p(gam))
-        got = ops.gamma(x.cuda(), gam.cuda()).cpu()
+        got = ops.intensity_fused(x.cuda(), gamma=gam.cuda()).cpu()
         assert (got - want).abs().max() <= 2e-6
         assert torch.equal(got[1], x[1])
 
 
 def test_philox_noise_statistics():
+    """The Philox stream Noise uses under TIO_B200_NOISE=philox (noise_mode 2)."""
     from torchio_b200 import ops
 
     x = torch.zeros((2, 1, 64, 64, 64), device="cuda")
     mean = torch.tensor([0.5, -1.0], device="cuda")
     std = torch.tensor([2.0, 0.5], device="cuda")
-    y = ops.noise_philox(x, mean, std, None, seed=1234).cpu()
+
+    def philox(seed):
+        return ops.intensity_fused(x, mean=mean, std=std, noise_mode=2, philox_seed=seed).cpu()
+
+    y = philox(1234)
     for b in range(2):
         assert abs(float(y[b].mean()) - float(mean[b])) < 0.02 * float(std[b]) + 1e-3
         assert abs(float(y[b].std()) - float(std[b])) < 0.01 * float(std[b])
-    y2 = ops.noise_philox(x, mean, std, None, seed=1234).cpu()
+    y2 = philox(1234)
     assert torch.equal(y, y2)
-    y3 = ops.noise_philox(x, mean, std, None, seed=1235).cpu()
+    y3 = philox(1235)
     assert not torch.equal(y, y3)
     kurt = float(((y[0] - y[0].mean()) ** 4).mean() / y[0].var() ** 2)
     assert abs(kurt - 3.0) < 0.05

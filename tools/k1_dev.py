@@ -121,8 +121,7 @@ def time_all(b):
                 ms = timeit(lambda: ops.resample(x, mat, cps, flags, one, one, affine_first=True, mode=ops.LINEAR,
                                                  fill=fill, box_hint=hint, exact_coords=exact))
                 print(f"TIME {name:8s} box={hint} {'exact' if exact else 'fast '} {ms:.3f} ms  "
-                      f"{1e3 * gb / ms:.0f} GB/s  reuse={os.environ.get('TIO_B200_K1_REUSE', '1')}"
-                      f" prefetch={os.environ.get('TIO_B200_K1_PREFETCH', 'default')}", flush=True)
+                      f"{1e3 * gb / ms:.0f} GB/s", flush=True)
     del y
 
 

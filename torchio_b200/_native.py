@@ -25,14 +25,8 @@ _SIGNATURES = {
     "tio_upload": [c_void_p, c_void_p, c_size_t, c_void_p],
     "tio_remap": [c_void_p, c_void_p, c_int] + [c_int] * 8 + [c_int] * 3 + [c_int, c_void_p, c_void_p, c_void_p],
     "tio_crop_patches": [c_void_p, c_void_p, c_int] + [c_int] * 5 + [c_void_p, c_int, c_int, c_int, c_void_p],
-    "tio_bias_field": [c_void_p, c_void_p] + [c_int] * 5 + [c_void_p] + [c_int] * 3
-    + [c_void_p, c_int, c_void_p],
     "tio_blur": [c_void_p, c_void_p, c_void_p] + [c_int] * 5
     + [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p],
-    "tio_noise": [c_void_p, c_void_p, c_int, c_int64] + [c_void_p] * 6,
-    "tio_noise_philox": [c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p, c_void_p,
-                         c_uint64, c_int, c_void_p],
-    "tio_gamma": [c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p],
     "tio_moments": [c_void_p, c_void_p, c_int64, c_void_p, c_void_p],
     "tio_quantiles_workspace_bytes": [],
     "tio_quantiles": [c_void_p, c_void_p, c_int64, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p,

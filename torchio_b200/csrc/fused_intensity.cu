@@ -17,10 +17,54 @@
 // Separable passes commute up to fp32 summation order (the reference runs
 // I, J, K; this runs I, K, J): differences are ~1e-7 relative.
 #include "common.cuh"
-#include "intensity_common.cuh"
 #include "tma.cuh"
 
 namespace tio {
+
+__device__ __forceinline__ float rician(float x, float n1, float n2) {
+  float s = __fadd_rn(x, n1);
+  return sqrtf(__fadd_rn(__fmul_rn(s, s), __fmul_rn(n2, n2)));
+}
+
+
+// Philox4x32 (Salmon et al. 2011), 7 rounds (the paper's Crush-resistant minimum;
+// the name is kept for the call sites), counter = element-group index.
+__device__ __forceinline__ uint4 philox4x32_10(uint4 ctr, uint2 key) {
+  const uint32_t M0 = 0xD2511F53u, M1 = 0xCD9E8D57u, W0 = 0x9E3779B9u, W1 = 0xBB67AE85u;
+#pragma unroll
+  for (int r = 0; r < 7; ++r) {
+    uint32_t hi0 = __umulhi(M0, ctr.x), lo0 = M0 * ctr.x;
+    uint32_t hi1 = __umulhi(M1, ctr.z), lo1 = M1 * ctr.z;
+    ctr = make_uint4(hi1 ^ ctr.y ^ key.x, lo1, hi0 ^ ctr.w ^ key.y, lo0);
+    key.x += W0;
+    key.y += W1;
+  }
+  return ctr;
+}
+
+__device__ __forceinline__ void box_muller(uint32_t a, uint32_t b, float& n0, float& n1) {
+  float u1 = ((float)(a >> 8) + 0.5f) * (1.0f / 16777216.0f);  // (0,1)
+  float u2 = ((float)(b >> 8)) * (1.0f / 16777216.0f);
+  float rad;
+  asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(rad) : "f"(-2.0f * __logf(u1)));
+  float s, c;
+  __sincosf(6.283185307179586f * u2, &s, &c);
+  n0 = rad * c;
+  n1 = rad * s;
+}
+
+
+__device__ __forceinline__ float signed_pow(float x, float gam) {
+  // sign(x) * |x|^gamma (gamma.py:88-90); gamma == 1 -> x exactly (gated rows).
+  // |x|^g = 2^(g*log2|x|) on the SFU (lg2/ex2.approx): ~3e-7 relative for the
+  // value ranges of normalised images, far inside the 1e-4 parity tolerance.
+  if (gam == 1.0f) return x;
+  float ax = fabsf(x);
+  float p;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(p) : "f"(gam * __log2f(ax)));
+  p = ax == 0.0f ? 0.0f : p;
+  return x < 0.0f ? -p : p;
+}
 
 constexpr int A_TJ = 32;
 constexpr int A_TK = 64;

@@ -6,8 +6,6 @@
 // data/batch.py:52-58).  On the device one launch gathers all `n` patches of a
 // volume into a dense (n, C, pi, pj, pk) block, reading every source byte once.
 // Pure data movement: bound by HBM, algorithmic bytes = 2 x patch bytes.
-#include <cstdlib>
-
 #include "common.cuh"
 
 namespace tio {
@@ -219,11 +217,7 @@ static void launch_remap(const void* src, void* dst, int B, int C, int I, int J,
   memcpy(&fill, &fill_bits, sizeof(T));
   const long long rows = (long long)B * C * OI * OJ;
   constexpr int V = 16 / (int)sizeof(T);
-  static const bool scalar_only = []() {  // TIO_B200_REMAP_SCALAR=1: development knob (A/B timing)
-    const char* e = getenv("TIO_B200_REMAP_SCALAR");
-    return e && e[0] == '1';
-  }();
-  if (!scalar_only && OK % V == 0 && ((uintptr_t)dst & 15) == 0 && rows * (OK / V) / 256 < (1ll << 31)) {
+  if (OK % V == 0 && ((uintptr_t)dst & 15) == 0 && rows * (OK / V) / 256 < (1ll << 31)) {
     const long long units = rows * (OK / V);
     remap_vec_kernel<T><<<(unsigned)((units + 255) / 256), 256, 0, st>>>(
         (const T*)src, (T*)dst, B, C, I, J, K, OI, OJ, OK, oi, oj, ok, mode, fill, flip, units);

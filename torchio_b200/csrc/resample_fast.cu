@@ -21,7 +21,6 @@
 // within 1e-3 of the threshold are recomputed by the exact general column of
 // resample_common.cuh, so fill decisions stay bit-exact.  Label maps, nearest interpolation
 // and TIO_EXACT_COORDS launches use resample_tile.cu.
-#include <cstdlib>
 #include <type_traits>
 
 #include "resample_tile.cuh"
@@ -197,7 +196,9 @@ __device__ __forceinline__ void pair_step(const f2 rel2, const f2 A0, const f2 A
   }
 }
 
-template <int BOX, bool HAS_CP, bool HAS_FILL, bool REUSE>
+// Affine launches keep the upper-plane taps in registers along the walk (Carry); elastic launches
+// load all eight taps of every voxel.
+template <int BOX, bool HAS_CP, bool HAS_FILL>
 __global__ void __launch_bounds__(256, BOX <= 22 ? 4 : 3)
 resample_fast_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap tmap_s,
                      const __grid_constant__ ResampleArgs a, const __grid_constant__ TileArgs ta,
@@ -236,21 +237,6 @@ resample_fast_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_cons
     mbar_fence_init();
     mbar_expect_tx(bar, (uint32_t)((small ? NBOXS : NBOX) * 4));
     tma_load_4d(box_u32, small ? &tmap_s : &tmap, rec.z, rec.y, rec.x, b * a.C, bar);
-  }
-  // The CTA that will run ~one resident wave later finds its box in L2 instead of waiting at the
-  // barrier behind its TMA load for the HBM latency of the part of the box no neighbouring tile
-  // has touched yet.  Elastic launches only, and only when TIO_B200_K1_PREFETCH sets a distance
-  // (off by default, see launch_resample_tile).
-  if (HAS_CP && ta.prefetch_ahead && tid == 224) {
-    const unsigned ahead = tile_id + ta.prefetch_ahead;
-    if (ahead < gridDim.x * gridDim.y * gridDim.z) {
-      const int4 nxt = __ldg(records + ahead);
-      if ((nxt.w & (255 | 2048)) == (1 | 2048)) {
-        const unsigned z2 = ahead / (gridDim.x * gridDim.y);
-        const int b2 = tiles_i == 1 ? (int)z2 : (int)__umulhi(z2, ta.inv_tiles_i);
-        tma_prefetch_4d((DUAL && (nxt.w & 4096)) ? &tmap_s : &tmap, nxt.z, nxt.y, nxt.x, b2 * a.C);
-      }
-    }
   }
   const bool elastic = HAS_CP && (rec.w & 1024);
   const bool masked = HAS_FILL && !(rec.w & 256);  // some tap of the tile may leave the volume
@@ -393,8 +379,8 @@ resample_fast_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_cons
       for (int q = 0; q < count; ++q) {
         float va, vb;
         bool unc_a = false, unc_b = false;
-        pair_step<SMALL ? C1S : C1, SMALL ? C2S : C2, MASKED, REUSE>(rel2, A0, A1, A2, B0, B1, B2, kb, tz, fill_c,
-                                                                       va, vb, unc_a, unc_b, carry);
+        pair_step<SMALL ? C1S : C1, SMALL ? C2S : C2, MASKED, !HAS_CP>(rel2, A0, A1, A2, B0, B1, B2, kb, tz, fill_c,
+                                                                         va, vb, unc_a, unc_b, carry);
         *reinterpret_cast<float*>(out_a) = va;
         *reinterpret_cast<float*>(out_b) = vb;
         if (MASKED) {
@@ -440,9 +426,9 @@ resample_fast_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_cons
         float va, vb;
         bool unc_a = false, unc_b = false;
         if (masked)
-          pair_step<C1, C2, true, REUSE>(rel2, A0, A1, A2, B0, B1, B2, kb, tz, fill_c, va, vb, unc_a, unc_b, carry);
+          pair_step<C1, C2, true, !HAS_CP>(rel2, A0, A1, A2, B0, B1, B2, kb, tz, fill_c, va, vb, unc_a, unc_b, carry);
         else
-          pair_step<C1, C2, false, REUSE>(rel2, A0, A1, A2, B0, B1, B2, kb, tz, fill_c, va, vb, unc_a, unc_b, carry);
+          pair_step<C1, C2, false, !HAS_CP>(rel2, A0, A1, A2, B0, B1, B2, kb, tz, fill_c, va, vb, unc_a, unc_b, carry);
         *reinterpret_cast<float*>(out_a) = va;
         *reinterpret_cast<float*>(out_b) = vb;
         if (HAS_FILL) {
@@ -459,47 +445,36 @@ resample_fast_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_cons
   if (HAS_FILL && unsafe) exact_fix<HAS_CP, HAS_FILL>(a, ta, b, elastic, i0, unsafe, j0 + jrow, k0 + kcol);
 }
 
-template <int BOX, bool HAS_CP, bool REUSE>
-static void launch_fast_r(const CUtensorMap& tm, const CUtensorMap& tms, const ResampleArgs& a, const TileArgs& ta,
-                          dim3 grid, size_t smem, const int4* records, cudaStream_t st) {
+template <int BOX, bool HAS_CP>
+static void launch_fast_cp(const CUtensorMap& tm, const CUtensorMap& tms, const ResampleArgs& a, const TileArgs& ta,
+                           dim3 grid, size_t smem, const int4* records, cudaStream_t st) {
   if (a.fill) {
-    cudaFuncSetAttribute(resample_fast_kernel<BOX, HAS_CP, true, REUSE>,
-                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    resample_fast_kernel<BOX, HAS_CP, true, REUSE><<<grid, 256, smem, st>>>(tm, tms, a, ta, records);
+    cudaFuncSetAttribute(resample_fast_kernel<BOX, HAS_CP, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                         (int)smem);
+    resample_fast_kernel<BOX, HAS_CP, true><<<grid, 256, smem, st>>>(tm, tms, a, ta, records);
   } else {
-    cudaFuncSetAttribute(resample_fast_kernel<BOX, HAS_CP, false, REUSE>,
-                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    resample_fast_kernel<BOX, HAS_CP, false, REUSE><<<grid, 256, smem, st>>>(tm, tms, a, ta, records);
+    cudaFuncSetAttribute(resample_fast_kernel<BOX, HAS_CP, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                         (int)smem);
+    resample_fast_kernel<BOX, HAS_CP, false><<<grid, 256, smem, st>>>(tm, tms, a, ta, records);
   }
 }
 
 template <int BOX>
 static void launch_fast(const CUtensorMap& tm, const CUtensorMap& tms, const ResampleArgs& a, const TileArgs& ta,
-                        dim3 grid, size_t smem, int reuse, const int4* records, cudaStream_t st) {
-  // bit 0: affine-only launches, bit 1: launches with a control grid
-  if (a.cp) {
-    if (reuse & 2) launch_fast_r<BOX, true, true>(tm, tms, a, ta, grid, smem, records, st);
-    else launch_fast_r<BOX, true, false>(tm, tms, a, ta, grid, smem, records, st);
-  } else {
-    if (reuse & 1) launch_fast_r<BOX, false, true>(tm, tms, a, ta, grid, smem, records, st);
-    else launch_fast_r<BOX, false, false>(tm, tms, a, ta, grid, smem, records, st);
-  }
+                        dim3 grid, size_t smem, const int4* records, cudaStream_t st) {
+  if (a.cp) launch_fast_cp<BOX, true>(tm, tms, a, ta, grid, smem, records, st);
+  else launch_fast_cp<BOX, false>(tm, tms, a, ta, grid, smem, records, st);
 }
 
 // fp32 + trilinear tiles of the launch prepared by launch_resample_tile (tensor map, tile
-// arguments, bounds records).  TIO_B200_K1_REUSE (development knob, default 1): bit 0 / bit 1 =
-// keep the upper-plane taps in registers along the walk for affine / elastic launches.
+// arguments, bounds records)
 void launch_resample_fast(int box, const CUtensorMap& tm, const CUtensorMap& tm_small, const ResampleArgs& a,
                           const TileArgs& ta, dim3 grid, size_t smem, const int4* records, cudaStream_t st) {
-  static const int reuse = []() {
-    const char* e = getenv("TIO_B200_K1_REUSE");
-    return e ? atoi(e) & 3 : 1;
-  }();
-  if (box == 20) launch_fast<20>(tm, tm_small, a, ta, grid, smem, reuse, records, st);
-  else if (box == 22) launch_fast<22>(tm, tm_small, a, ta, grid, smem, reuse, records, st);
-  else if (box == 24) launch_fast<24>(tm, tm_small, a, ta, grid, smem, reuse, records, st);
-  else if (box == 28) launch_fast<28>(tm, tm_small, a, ta, grid, smem, reuse, records, st);
-  else launch_fast<32>(tm, tm_small, a, ta, grid, smem, reuse, records, st);
+  if (box == 20) launch_fast<20>(tm, tm_small, a, ta, grid, smem, records, st);
+  else if (box == 22) launch_fast<22>(tm, tm_small, a, ta, grid, smem, records, st);
+  else if (box == 24) launch_fast<24>(tm, tm_small, a, ta, grid, smem, records, st);
+  else if (box == 28) launch_fast<28>(tm, tm_small, a, ta, grid, smem, records, st);
+  else launch_fast<32>(tm, tm_small, a, ta, grid, smem, records, st);
 }
 
 }  // namespace tio

@@ -20,7 +20,6 @@
 // uses FMA lerps (<= 1 ulp from the reference's mul+add chain).
 #include <cuda.h>
 
-#include <cstdlib>
 #include <map>
 #include <mutex>
 
@@ -693,15 +692,6 @@ int launch_resample_tile(const ResampleArgs& a, int dtype, int mode, bool exact_
   ta.sp_in_one = (a.sp_in[0] == 1.f && a.sp_in[1] == 1.f && a.sp_in[2] == 1.f);
   ta.sp_out_one = (a.sp_out[0] == 1.f && a.sp_out[1] == 1.f && a.sp_out[2] == 1.f);
   ta.magic_bytes = (unsigned)kMagicBits << 2;
-  {  // TIO_B200_K1_PREFETCH: tiles of look-ahead of the L2 box prefetch (development knob).  Off by
-     // default: on an H100 SXM at 400 W every distance tried (99, 198, 396 tiles) made the K1
-     // launches slower than none (2.93-3.00 vs 2.70 ms per 32 x 256^3 launch, affine + elastic mean).
-    static const int ahead = []() {
-      const char* e = getenv("TIO_B200_K1_PREFETCH");
-      return e ? atoi(e) : 0;
-    }();
-    ta.prefetch_ahead = ahead > 0 ? (unsigned)ahead : 0u;
-  }
   for (int t = 0; t < 3; ++t) {
     ta.rsp_in[t] = (float)(1.0 / (double)a.sp_in[t]);
     ta.rsp_out[t] = (float)(1.0 / (double)a.sp_out[t]);

@@ -31,7 +31,6 @@ struct TileArgs {
   long long n_in, n_out;      // voxels per input / output channel
   int tiles_i;                // output tiles along I
   unsigned inv_tiles_i;       // floor(2^32 / tiles_i) + 1: z / tiles_i == umulhi(z, inv) for z < 2^16
-  unsigned prefetch_ahead;    // fast kernel: L2-prefetch the box of the tile this many tiles later (0 = off)
 };
 
 template <int OFFSET>

@@ -70,13 +70,4 @@ __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* tm,
       : "memory");
 }
 
-// pull the lines of a box into L2 ahead of the load that will stage it (no shared-memory
-// destination, no completion to wait for)
-__device__ __forceinline__ void tma_prefetch_4d(const CUtensorMap* tm, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.prefetch.tensor.4d.L2.global.tile [%0, {%1, %2, %3, %4}];" ::"l"(
-                   (unsigned long long)tm),
-               "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
-
 }  // namespace tio

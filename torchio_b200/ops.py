@@ -338,23 +338,6 @@ def remap(src: Tensor, out_shape, offsets, *, mode: str = "constant", fill=0, fl
     return dst
 
 
-def bias_field(src: Tensor, coarse: Tensor, identity: Tensor | None, *, divide=False,
-               out: Tensor | None = None) -> Tensor:
-    """K2 (intensity/bias_field.py:201-255,296-341)."""
-    _require_cuda(src, "bias_field")
-    src = src.contiguous()
-    b, c, i, j, k = src.shape
-    dst = torch.empty_like(src) if out is None else out
-    si, sj, sk = coarse.shape[2:]
-    with torch.cuda.device(src.device):
-        _native.call(
-            "tio_bias_field", _ptr(src), _ptr(dst), b, c, i, j, k, _ptr(coarse), si, sj, sk,
-            _ptr(identity), int(bool(divide)), _stream(src),
-        )
-    _count(1)
-    return dst
-
-
 def blur(src: Tensor, taps: Tensor, radius: Tensor, big_r: int, axes_mask: int,
          identity: Tensor | None) -> Tensor:
     """K3 (intensity/blur.py:129-252)."""
@@ -376,50 +359,6 @@ def _fused_launches(axes_mask: int, has_bias: bool) -> int:
     jk = bool(axes_mask & 6)
     march = (not jk) or bool(axes_mask & 1) or has_bias
     return int(jk) + int(march)
-
-
-def noise(src: Tensor, mean: Tensor, std: Tensor, keep: Tensor | None, z: Tensor,
-          z2: Tensor | None = None) -> Tensor:
-    """K4 with caller-provided normals (intensity/noise.py:98-178)."""
-    _require_cuda(src, "noise")
-    src = src.contiguous()
-    dst = torch.empty_like(src)
-    with torch.cuda.device(src.device):
-        _native.call(
-            "tio_noise", _ptr(src), _ptr(dst), src.shape[0], src[0].numel(), _ptr(mean),
-            _ptr(std), _ptr(keep), _ptr(z), _ptr(z2), _stream(src),
-        )
-    _count(1)
-    return dst
-
-
-def noise_philox(src: Tensor, mean: Tensor, std: Tensor, keep: Tensor | None, seed: int,
-                 rician: bool = False) -> Tensor:
-    """K4b: in-register Philox normals (not the reference stream)."""
-    _require_cuda(src, "noise_philox")
-    src = src.contiguous()
-    dst = torch.empty_like(src)
-    with torch.cuda.device(src.device):
-        _native.call(
-            "tio_noise_philox", _ptr(src), _ptr(dst), src.shape[0], src[0].numel(),
-            _ptr(mean), _ptr(std), _ptr(keep), int(seed), int(bool(rician)), _stream(src),
-        )
-    _count(1)
-    return dst
-
-
-def gamma(src: Tensor, gam: Tensor) -> Tensor:
-    """K5 (intensity/gamma.py:88-90)."""
-    _require_cuda(src, "gamma")
-    src = src.contiguous()
-    dst = torch.empty_like(src)
-    with torch.cuda.device(src.device):
-        _native.call(
-            "tio_gamma", _ptr(src), _ptr(dst), src.shape[0], src[0].numel(), _ptr(gam),
-            _stream(src),
-        )
-    _count(1)
-    return dst
 
 
 def moments(values: Tensor, mask: Tensor | None = None) -> tuple[float, float, float]:
@@ -497,8 +436,8 @@ def intensity_fused(
 ) -> Tensor:
     """Fused bias -> blur -> noise -> gamma (two HBM passes); any stage optional.
 
-    Compose-level fusion of consecutive intensity transforms; equal to running
-    `bias_field`, `blur`, `noise`, `gamma` in sequence up to fp32 summation order.
+    Compose-level fusion of consecutive intensity transforms; a single transform
+    is a call with only its own stage set.
     """
     _require_cuda(src, "intensity_fused")
     src = src.contiguous()
