@@ -276,6 +276,27 @@ int tio_intensity_fused(const float* src, float* dst, float* scratch,
                         uint64_t philox_seed, int noise_mode, int rician,
                         const float* gamma, void* stream);
 
+/*
+ * LabelsToImage in one pass: dst (B, 1, vox) fp32 from channel 0 of `labels` (B, C, vox) of
+ * `dtype`.  Replaces _generate_from_labels / _generate_per_element
+ * (transforms/intensity/labels_to_image.py:182-290): per drawn label, in the reference's order,
+ * result += (torch.randn_like(result) * std + mean) * (label == l) on a CUDA batch.
+ *   label_values  [n] device int64, strictly ascending; a voxel matches l when `label == int(l)`
+ *                 (fp32 maps: integral values only), n <= 2048
+ *   mean, std     [B][n] device fp32 (per element; the shared form repeats one row)
+ *   draw_offset   [n] device uint64: the Philox offset ATen's normal kernel would have been handed
+ *                 for that label's randn_like draw, or ~0 when the label is not drawn
+ *   seed          the CUDA generator's seed; grid_x the block count of ATen's launch
+ *                 (min(SMs * maxThreadsPerSM / 256, ceil(B*vox / 256)))
+ * Each voxel of a drawn label l is (((z + 0) * std) + mean) + 0 rounded step by step, z the
+ * element ATen's draw wrote there; every other voxel is +0.  B*vox <= 2^29 (ATen splits larger
+ * draws into several launches with other offsets).
+ */
+int tio_labels_to_image(const void* labels, int dtype, int C, int B, int64_t vox,
+                        const int64_t* label_values, int n, const float* mean, const float* std,
+                        const uint64_t* draw_offset, uint64_t seed, int grid_x, float* dst,
+                        void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,8 +1,8 @@
 """torchio_b200 — CUDA-native 3-D augmentation hot path behind the TorchIO v2 API.
 
 Drop-in for the reference's spatial + intensity augmentation chain
-(`Affine`, `ElasticDeformation`, `Spatial`, `BiasField`, `Blur`, `Noise`,
-`Gamma`, `Compose`) and its patch path (`UniformSampler`, `Queue`,
+(`Affine`, `ElasticDeformation`, `Spatial`, `LabelsToImage`, `BiasField`, `Blur`,
+`Noise`, `Gamma`, `Compose`) and its patch path (`UniformSampler`, `Queue`,
 `SubjectsLoader`) on tensor-backed `Subject` / `SubjectsBatch` data.  The
 tensor math runs in hand-written sm_90a (H100) CUDA kernels exposed through the C-ABI
 of ``include/tio_b200.h``; see DESIGN.md and INTEGRATION.md.
@@ -16,7 +16,7 @@ from .patches import (GridSampler, ImagesLoader, LabelSampler, PatchLocation, Pa
                       StudiesLoader, SubjectsLoader, UniformSampler, WeightedSampler, collate_images, collate_studies,
                       collate_subjects)
 from .transforms import (Affine, AppliedTransform, BiasField, Blur, Compose, Crop, CropOrPad,
-                         ElasticDeformation, Flip, Gamma, IntensityTransform, Noise, Normalize, Pad, Resample, RescaleIntensity, Spatial,
+                         ElasticDeformation, Flip, Gamma, IntensityTransform, LabelsToImage, Noise, Normalize, Pad, Resample, RescaleIntensity, Spatial,
                          SpatialTransform, Standardize, Transform,
                          apply_inverse_transform, execution_device, get_inverse_transform,
                          set_execution_device)
@@ -26,7 +26,7 @@ __version__ = "0.1.0"
 __all__ = [
     "Affine", "AffineMatrix", "AppliedTransform", "BiasField", "Blur", "Choice", "Compose", "Crop", "CropOrPad",
     "ElasticDeformation", "Flip", "Gamma", "GridSampler", "Image", "ImagesBatch", "ImagesLoader", "IntensityTransform",
-    "LabelMap", "LabelSampler", "Noise", "Normalize", "Pad", "PatchLocation", "PatchSampler", "Queue", "Resample", "RescaleIntensity", "ScalarImage", "Spatial",
+    "LabelMap", "LabelSampler", "LabelsToImage", "Noise", "Normalize", "Pad", "PatchLocation", "PatchSampler", "Queue", "Resample", "RescaleIntensity", "ScalarImage", "Spatial",
     "SpatialTransform", "Standardize", "StudiesBatch", "StudiesLoader", "Subject", "SubjectsBatch",
     "SubjectsLoader", "Transform", "UniformSampler", "WeightedSampler", "apply_inverse_transform", "collate_images",
     "collate_studies", "collate_subjects", "exact_coords_default", "execution_device", "get_inverse_transform",

@@ -44,6 +44,8 @@ _SIGNATURES = {
     + [c_void_p, c_int, c_int, c_int, c_void_p, c_int]
     + [c_void_p, c_void_p, c_int, c_int]
     + [c_void_p] * 5 + [c_uint64, c_int, c_int, c_void_p, c_void_p],
+    "tio_labels_to_image": [c_void_p, c_int, c_int, c_int, c_int64, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
+                            c_uint64, c_int, c_void_p, c_void_p],
 }
 
 _lib = None

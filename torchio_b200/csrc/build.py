@@ -18,7 +18,7 @@ from pathlib import Path
 HERE = Path(__file__).resolve().parent
 ROOT = HERE.parent.parent
 SOURCES = ["error.cu", "resample.cu", "resample_tile.cu", "resample_fast.cu", "upload.cu", "fused_intensity.cu",
-           "mt19937_jump.cpp", "mt19937.cu", "patches.cu", "stats.cu", "labels.cu"]
+           "mt19937_jump.cpp", "mt19937.cu", "patches.cu", "stats.cu", "labels.cu", "labels_to_image.cu"]
 HEADERS = [HERE / "common.cuh", HERE / "resample_common.cuh", HERE / "resample_tile.cuh", HERE / "tma.cuh",
            HERE / "mt19937_layout.h",
            ROOT / "include" / "tio_b200.h",

@@ -16,7 +16,7 @@ import numpy as np
 import torch
 from torch import Tensor
 
-from . import _native
+from . import _native, tables
 
 DTYPE_CODES = {
     torch.float32: 0, torch.uint8: 1, torch.int8: 2,
@@ -529,3 +529,66 @@ def randn_mt19937(seed: int, offset: int, n: int, device, out: Tensor | None = N
                      _ptr(workspace), ws_bytes, torch.cuda.current_stream(device).cuda_stream)
     _count(4)
     return z
+
+
+# ---- LabelsToImage: the reference's CUDA randn_like draws, recomputed per voxel --------
+
+_cuda_rng_lock = threading.Lock()
+
+
+def labels_to_image(labels: Tensor, label_values, means, stds, draw=None) -> Tensor:
+    """(B, C, I, J, K) label batch -> (B, 1, I, J, K) fp32 synthetic image, bit-identical to
+    _generate_from_labels / _generate_per_element (intensity/labels_to_image.py:182-290) run on
+    the same CUDA tensors from the same CUDA generator state, which it advances by as much.
+
+    ``label_values``: ascending distinct labels; ``means`` / ``stds``: (B, n) or (n,) values per
+    label; ``draw``: (n,) position of each label in the reference's draw order, -1 = no draw
+    (default: ascending order, skipping labels whose means and stds are all zero).  Channel 0 is
+    read.  One draw of B*I*J*K normals per drawn label is reserved on the device's default CUDA
+    generator, as ATen's ``philox_cuda_state`` would hand them out."""
+    if labels.dtype not in DTYPE_CODES:
+        raise TypeError(f"labels_to_image: unsupported label dtype {labels.dtype}")
+    if labels.ndim != 5:
+        raise ValueError(f"labels_to_image expects (B, C, I, J, K), got {tuple(labels.shape)}")
+    b, c = int(labels.shape[0]), int(labels.shape[1])
+    vox = int(np.prod(labels.shape[2:]))
+    numel = b * vox
+    tables.check_randn_numel(numel)
+    _require_cuda(labels, "labels_to_image")
+    if torch.cuda.is_current_stream_capturing():
+        raise RuntimeError("labels_to_image: CUDA-graph capture is not supported (the generator offsets are"
+                           " reserved on the host)")
+    values = np.ascontiguousarray(np.asarray(label_values, dtype=np.int64).reshape(-1))
+    n = int(values.shape[0])
+    if n and np.any(np.diff(values) <= 0):
+        raise ValueError("labels_to_image: label_values must be strictly ascending")
+    mean = np.array(np.broadcast_to(np.asarray(means, dtype=np.float32).reshape(-1, n), (b, n)))
+    std = np.array(np.broadcast_to(np.asarray(stds, dtype=np.float32).reshape(-1, n), (b, n)))
+    if draw is None:
+        active = np.any(mean != 0, axis=0) | np.any(std != 0, axis=0)
+        draw = np.where(active, np.cumsum(active) - 1, -1)
+    draw = np.asarray(draw, dtype=np.int64).reshape(n)
+    n_draws = int((draw >= 0).sum())
+    out = torch.empty((b, 1, *labels.shape[2:]), dtype=torch.float32, device=labels.device)
+    if numel == 0:
+        return out  # randn_like of an empty tensor consumes nothing
+    device = labels.device
+    props = torch.cuda.get_device_properties(device)
+    grid_x, counter_offset = tables.randn_cuda_layout(numel, props.multi_processor_count,
+                                                      props.max_threads_per_multi_processor)
+    gen = torch.cuda.default_generators[device.index]
+    with _cuda_rng_lock:
+        seed = int(gen.initial_seed())
+        base = int(gen.get_offset())
+        if n_draws:
+            gen.set_offset(base + n_draws * counter_offset)
+    # draw k starts where the k previous draws left the offset; -1 (all bits set) = not drawn
+    offsets = np.where(draw >= 0, base + draw * counter_offset, -1).astype(np.int64)
+    labels = labels.contiguous()
+    values_d, mean_d, std_d, offsets_d = upload(device, values, mean, std, offsets) if n else (None,) * 4
+    with torch.cuda.device(device):
+        _native.call("tio_labels_to_image", _ptr(labels), DTYPE_CODES[labels.dtype], c, b, vox, _ptr(values_d), n,
+                     _ptr(mean_d), _ptr(std_d), _ptr(offsets_d), seed & (2**64 - 1), grid_x, _ptr(out),
+                     _stream(labels))
+    _count(2 if n else 1)
+    return out

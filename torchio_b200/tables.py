@@ -219,3 +219,73 @@ def gamma_values(log_gamma, batch_size: int) -> np.ndarray:
             )
         return torch.exp(torch.tensor(log_gamma, dtype=torch.float32)).numpy()
     return np.full(batch_size, math.exp(log_gamma), dtype=np.float32)
+
+
+# ---- labels to image -----------------------------------------------------------
+
+#: Largest draw ATen's CUDA normal kernel runs as a single launch: TensorIterator's
+#: can_use_32bit_indexing needs the last fp32 byte offset to fit in int32, i.e. numel <= 2**29.
+#: Larger draws are split into sub-launches, each with an offset of its own.
+RANDN_MAX_NUMEL = 1 << 29
+
+
+def check_randn_numel(numel: int) -> None:
+    if numel > RANDN_MAX_NUMEL:
+        raise NotImplementedError(
+            f"a draw of {numel} values exceeds 2**29; ATen splits it into 32-bit-indexed"
+            " sub-launches, whose stream is not reproduced")
+
+
+def randn_cuda_layout(numel: int, sm_count: int, max_threads_per_sm: int) -> tuple[int, int]:
+    """(grid_x, counter_offset) of ATen's launch of ``normal_`` on ``numel`` fp32 CUDA values
+    (calc_execution_policy, ATen/native/cuda/DistributionTemplates.h: 256-thread blocks, 4 values
+    per curand_normal4).  ``counter_offset`` is how far the draw advances the generator's offset."""
+    if numel < 1:
+        raise ValueError(f"randn_cuda_layout: numel must be positive, got {numel}")
+    check_randn_numel(numel)
+    block = 256
+    grid_x = min(sm_count * (max_threads_per_sm // block), (numel + block - 1) // block)
+    counter_offset = ((numel - 1) // (block * grid_x * 4) + 1) * 4
+    return grid_x, counter_offset
+
+
+def label_synthesis_tables(means, stds, batch_size: int):
+    """LabelsToImage params -> (label values (n,) int64 ascending, draw index (n,) int64 with -1 for
+    a label that is not drawn, mean (B, n) fp32, std (B, n) fp32).
+
+    Draw order is the reference's: the ``means`` dict's order for shared params
+    (labels_to_image.py:282-285), the sorted union of the per-element dicts otherwise (:201-213).
+    A label draws nothing when its mean and std are all zero (:212, :284).  Keys may be ints or,
+    for params read back from JSON, their strings."""
+    per_element = isinstance(means, list)
+    if per_element:
+        if len(means) != batch_size or len(stds) != batch_size:
+            raise RuntimeError(f"Per-instance parameters were recorded for {len(means)} elements"
+                               f" but the batch has {batch_size}")
+        m_rows = [{int(k): float(v) for k, v in m.items()} for m in means]
+        s_rows = [{int(k): float(v) for k, v in s.items()} for s in stds]
+        order = sorted(set().union(*(m.keys() for m in m_rows)))
+    else:
+        m_rows = [{int(k): float(v) for k, v in means.items()}] * batch_size
+        s_rows = [{int(k): float(v) for k, v in stds.items()}] * batch_size
+        order = list(m_rows[0])
+    values = np.asarray(sorted(order), dtype=np.int64)
+    column = {int(v): i for i, v in enumerate(values)}
+    mean = np.zeros((batch_size, len(values)), dtype=np.float32)
+    std = np.zeros_like(mean)
+    for b in range(batch_size):
+        for label in order:
+            mean[b, column[label]] = m_rows[b].get(label, 0.0)
+            std[b, column[label]] = s_rows[b].get(label, 0.0)
+    draw = np.full(len(values), -1, dtype=np.int64)
+    drawn = 0
+    for label in order:
+        c = column[label]
+        if per_element:  # count_nonzero of the fp32 (B,) tensors
+            active = np.any(mean[:, c] != 0) or np.any(std[:, c] != 0)
+        else:  # python floats
+            active = m_rows[0][label] != 0.0 or s_rows[0].get(label, 0.0) != 0.0
+        if active:
+            draw[c] = drawn
+            drawn += 1
+    return values, draw, mean, std

@@ -95,8 +95,20 @@ def chunk_scope(info: ChunkInfo | None):
         _chunk_local.info = previous
 
 
+_staging_local = threading.local()
+
+
+def staged_derived(name: str, source: str) -> None:
+    """Register an image a transform adds to a staged batch (see `_Staging.derive`); a no-op when
+    the batch was not staged."""
+    staging = getattr(_staging_local, "active", None)
+    if staging is not None:
+        staging.derive(name, source)
+
+
 class _Staging:
-    """Move a CPU batch to the execution device and back, preserving pinning."""
+    """Move a CPU batch to the execution device and back, preserving pinning.  Images a transform
+    adds during the call are brought back like the image they were derived from."""
 
     def __init__(self, batch: SubjectsBatch) -> None:
         self.batch = batch
@@ -111,9 +123,18 @@ class _Staging:
             dev = dev or execution_device()
             self.origin[name] = (t.device, t.is_pinned())
             ib.data = t.to(dev, non_blocking=True)
+        self.previous = getattr(_staging_local, "active", None)
+        _staging_local.active = self
         return self.batch
 
+    def derive(self, name: str, source: str) -> None:
+        """Image ``name``, created on the device from image ``source``, goes back to where
+        ``source`` came from (device and pinning) when the call ends."""
+        if source in self.origin:
+            self.origin[name] = self.origin[source]
+
     def __exit__(self, exc_type, exc, tb):
+        _staging_local.active = self.previous
         if exc_type is not None or not self.origin:
             return False
         for name, (device, pinned) in self.origin.items():

@@ -1,4 +1,4 @@
-"""BiasField / Blur / Noise / Gamma behind the reference API.
+"""BiasField / Blur / Noise / Gamma / LabelsToImage behind the reference API.
 
 Host-side mirror of transforms/intensity/{bias_field,blur,noise,gamma}.py
 (TorchIO 2.0.0a2): constructor signatures, ``make_params`` RNG order and the
@@ -17,9 +17,9 @@ import torch
 from torch import Tensor
 
 from .. import ops, tables
-from ..data import SubjectsBatch
+from ..data import ImagesBatch, LabelMap, ScalarImage, SubjectsBatch
 from ..params import to_nonneg_range, to_range
-from .base import IntensityTransform, chunk_info
+from .base import IntensityTransform, Transform, chunk_info, staged_derived
 
 
 def _as_f32(data: Tensor) -> Tensor:
@@ -373,6 +373,97 @@ class _GammaInverse(IntensityTransform):
         lg = self._log_gamma
         _apply_gamma(self, batch, [-v for v in lg] if isinstance(lg, list) else -lg)
         return batch
+
+
+# ---- LabelsToImage (intensity/labels_to_image.py:19-290) ---------------------------------------
+
+
+class LabelsToImage(Transform):
+    """Synthetic image from a label map: per label, Gaussian tissue with a sampled mean and std,
+    added to the batch as a new `ScalarImage` under ``image_key`` (existing images are untouched).
+
+    ``make_params`` is the reference's (labels of batch element 0, RNG order, params schema).  The
+    image is one `ops.labels_to_image` pass that recomputes, per voxel, the element of the
+    reference's ``torch.randn_like`` draw on the label map's CUDA device that the voxel keeps: a
+    device-resident batch gives the reference's image bit for bit and advances the CUDA generator
+    as it does.  A host-resident batch is synthesised on the execution device from that device's
+    CUDA generator (the reference would draw from the CPU generator) and the image is returned on
+    the host, pinned when the label map is."""
+
+    def __init__(self, label_key: str | None = None, *, image_key: str = "image_from_labels", mean=None,
+                 std=None, default_mean=(0.1, 0.9), default_std=(0.01, 0.1), ignore_background: bool = False,
+                 **kwargs: Any) -> None:
+        super().__init__(**kwargs)
+        self.label_key = label_key
+        self.image_key = image_key
+        self.mean_ranges = [to_range(m) for m in mean] if mean is not None else None
+        self.std_ranges = [to_range(s) for s in std] if std is not None else None
+        self.default_mean = to_range(default_mean)
+        self.default_std = to_range(default_std)
+        self.ignore_background = ignore_background
+
+    @property
+    def supports_per_instance_params(self) -> bool:
+        return True
+
+    def make_params(self, batch: SubjectsBatch) -> dict[str, Any]:
+        _, label_batch = self._find_label_batch(batch)
+        unique = sorted(int(v) for v in label_batch.data[0].unique().tolist())
+        n = self._resolve_n(batch)
+        if n is None:
+            means, stds = self._sample_label_values(unique)
+            return {"means": means, "stds": stds}
+        means_list, stds_list = [], []
+        for _ in range(n):
+            means, stds = self._sample_label_values(unique)
+            means_list.append(means)
+            stds_list.append(stds)
+        params = {"means": means_list, "stds": stds_list}
+        self._tag_batched(params, batch, n, None, ["means", "stds"])
+        return params
+
+    def _sample_label_values(self, unique: list[int]) -> tuple[dict[int, float], dict[int, float]]:
+        """mean then std per label, in ascending order (labels_to_image.py:105-132)."""
+        means: dict[int, float] = {}
+        stds: dict[int, float] = {}
+        for idx, label in enumerate(unique):
+            if self.ignore_background and label == 0:
+                means[label] = 0.0
+                stds[label] = 0.0
+                continue
+            if self.mean_ranges is not None and idx < len(self.mean_ranges):
+                means[label] = self.mean_ranges[idx].sample_1d()
+            else:
+                means[label] = self.default_mean.sample_1d()
+            if self.std_ranges is not None and idx < len(self.std_ranges):
+                stds[label] = self.std_ranges[idx].sample_1d()
+            else:
+                stds[label] = abs(self.default_std.sample_1d())
+        return means, stds
+
+    def apply_transform(self, batch: SubjectsBatch, params: dict[str, Any]) -> SubjectsBatch:
+        name, label_batch = self._find_label_batch(batch)
+        data = label_batch.data
+        if not data.is_cuda:
+            from .base import execution_device
+
+            data = data.to(execution_device())
+        values, draw, mean, std = tables.label_synthesis_tables(params["means"], params["stds"], data.shape[0])
+        generated = ops.labels_to_image(data, values, mean, std, draw)
+        batch.images[self.image_key] = ImagesBatch(generated, label_batch.affines, image_class=ScalarImage)
+        staged_derived(self.image_key, name)
+        return batch
+
+    def _find_label_batch(self, batch: SubjectsBatch):
+        """(name, label map batch): ``label_key``, or the first `LabelMap` (labels_to_image.py:164-179)."""
+        if self.label_key is not None:
+            if self.label_key not in batch.images:
+                raise KeyError(f"Label key '{self.label_key}' not found. Available: {list(batch.images.keys())}")
+            return self.label_key, batch.images[self.label_key]
+        for name, img_batch in batch.images.items():
+            if issubclass(img_batch._image_class, LabelMap):
+                return name, img_batch
+        raise KeyError("No LabelMap found in the subject")
 
 
 # ---- Standardize / Normalize (intensity/standardize.py:17-170, normalize.py:35-369) -----------
