@@ -297,6 +297,46 @@ int tio_labels_to_image(const void* labels, int dtype, int C, int B, int64_t vox
                         const uint64_t* draw_offset, uint64_t seed, int grid_x, float* dst,
                         void* stream);
 
+/*
+ * Label-map utilities (transforms/label/ of the reference), one pass each.  Label dtypes are
+ * tio_dtype codes; `src` is never modified.
+ *
+ * tio_label_lut: dst[e] = the value of src[e]'s key in the table, for `count` elements of `dtype`
+ * (dst has the same dtype; in-place allowed).  Replaces the clone / zeros_like + one compare and one
+ * masked index_put per entry of RemapLabels (remap_labels.py:50-58), RemoveLabels
+ * (remove_labels.py:54-61), SequentialLabels (sequential_labels.py:53-61) and its inverse (:97-105).
+ *   keys      [n] device, strictly ascending: int64 for integer maps (each key a value of the dtype),
+ *             fp32 for fp32 maps (matched by value: -0 finds +0, NaN finds nothing)
+ *   values    [n] device, `dtype`: what an element equal to keys[i] becomes
+ *   identity  1: an element without a key is copied (RemapLabels); 0: it becomes 0 (zeros_like)
+ * 8-bit maps hold at most 256 keys.
+ *
+ * tio_label_contour: dst (volumes, I, J, K) fp32 = 1 where the minimum of float(v) over the 3x3x3
+ * neighbourhood (-1 outside the volume) differs from float(v) or is NaN, else 0; `src` is `volumes`
+ * contiguous (I, J, K) volumes (B*C) of `dtype`.  Replaces _extract_contour (contour.py:52-71).
+ *
+ * tio_onehot_classes: dst (B, num_classes, vox) fp32 one-hot of channel 0 of `src` (B, C, vox):
+ * channel c is 1 where long(v) == c (fp32: truncated as the device converts it; a class the dtype
+ * cannot hold stays 0).  Replaces data.long(), F.one_hot, permute, .float() (one_hot.py:58-69).
+ *
+ * tio_label_range: range[0], range[1] (device int64) = the minimum and maximum of long(v) over
+ * channel 0 of `src` (B, C, vox); what one_hot's range checks and num_classes=-1 read.
+ *
+ * tio_channel_argmax: dst (B, 1, vox) fp32 = the index of the first maximum over the C channels of
+ * `src` (B, C, vox) of `dtype`, a NaN counting as the maximum (torch.argmax(dim=1)).  Replaces
+ * _OneHotInverse (one_hot.py:87-97).
+ */
+int tio_label_lut(const void* src, void* dst, int dtype, int64_t count, const void* keys,
+                  const void* values, int n, int identity, void* stream);
+int tio_label_contour(const void* src, int dtype, int volumes, int I, int J, int K, float* dst,
+                      void* stream);
+int tio_onehot_classes(const void* src, int dtype, int B, int C, int64_t vox, int num_classes,
+                       float* dst, void* stream);
+int tio_label_range(const void* src, int dtype, int B, int C, int64_t vox, int64_t* range,
+                    void* stream);
+int tio_channel_argmax(const void* src, int dtype, int B, int C, int64_t vox, float* dst,
+                       void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -2,7 +2,8 @@
 
 Drop-in for the reference's spatial + intensity augmentation chain
 (`Affine`, `ElasticDeformation`, `Spatial`, `LabelsToImage`, `BiasField`, `Blur`,
-`Noise`, `Gamma`, `Compose`) and its patch path (`UniformSampler`, `Queue`,
+`Noise`, `Gamma`, `Compose`), the label-map utilities (`RemapLabels`, `RemoveLabels`,
+`SequentialLabels`, `OneHot`, `Contour`) and its patch path (`UniformSampler`, `Queue`,
 `SubjectsLoader`) on tensor-backed `Subject` / `SubjectsBatch` data.  The
 tensor math runs in hand-written sm_90a (H100) CUDA kernels exposed through the C-ABI
 of ``include/tio_b200.h``; see DESIGN.md and INTEGRATION.md.
@@ -15,8 +16,9 @@ from .params import Choice
 from .patches import (GridSampler, ImagesLoader, LabelSampler, PatchLocation, PatchSampler, Queue,
                       StudiesLoader, SubjectsLoader, UniformSampler, WeightedSampler, collate_images, collate_studies,
                       collate_subjects)
-from .transforms import (Affine, AppliedTransform, BiasField, Blur, Compose, Crop, CropOrPad,
-                         ElasticDeformation, Flip, Gamma, IntensityTransform, LabelsToImage, Noise, Normalize, Pad, Resample, RescaleIntensity, Spatial,
+from .transforms import (Affine, AppliedTransform, BiasField, Blur, Compose, Contour, Crop, CropOrPad,
+                         ElasticDeformation, Flip, Gamma, IntensityTransform, LabelsToImage, Noise, Normalize, OneHot, Pad,
+                         RemapLabels, RemoveLabels, Resample, RescaleIntensity, SequentialLabels, Spatial,
                          SpatialTransform, Standardize, Transform,
                          apply_inverse_transform, execution_device, get_inverse_transform,
                          set_execution_device)
@@ -24,9 +26,10 @@ from .transforms import (Affine, AppliedTransform, BiasField, Blur, Compose, Cro
 __version__ = "0.1.0"
 
 __all__ = [
-    "Affine", "AffineMatrix", "AppliedTransform", "BiasField", "Blur", "Choice", "Compose", "Crop", "CropOrPad",
+    "Affine", "AffineMatrix", "AppliedTransform", "BiasField", "Blur", "Choice", "Compose", "Contour", "Crop", "CropOrPad",
     "ElasticDeformation", "Flip", "Gamma", "GridSampler", "Image", "ImagesBatch", "ImagesLoader", "IntensityTransform",
-    "LabelMap", "LabelSampler", "LabelsToImage", "Noise", "Normalize", "Pad", "PatchLocation", "PatchSampler", "Queue", "Resample", "RescaleIntensity", "ScalarImage", "Spatial",
+    "LabelMap", "LabelSampler", "LabelsToImage", "Noise", "Normalize", "OneHot", "Pad", "PatchLocation", "PatchSampler", "Queue", "RemapLabels", "RemoveLabels",
+    "Resample", "RescaleIntensity", "ScalarImage", "SequentialLabels", "Spatial",
     "SpatialTransform", "Standardize", "StudiesBatch", "StudiesLoader", "Subject", "SubjectsBatch",
     "SubjectsLoader", "Transform", "UniformSampler", "WeightedSampler", "apply_inverse_transform", "collate_images",
     "collate_studies", "collate_subjects", "exact_coords_default", "execution_device", "get_inverse_transform",

@@ -46,6 +46,11 @@ _SIGNATURES = {
     + [c_void_p] * 5 + [c_uint64, c_int, c_int, c_void_p, c_void_p],
     "tio_labels_to_image": [c_void_p, c_int, c_int, c_int, c_int64, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
                             c_uint64, c_int, c_void_p, c_void_p],
+    "tio_label_lut": [c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p, c_int, c_int, c_void_p],
+    "tio_label_contour": [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p],
+    "tio_onehot_classes": [c_void_p, c_int, c_int, c_int, c_int64, c_int, c_void_p, c_void_p],
+    "tio_label_range": [c_void_p, c_int, c_int, c_int, c_int64, c_void_p, c_void_p],
+    "tio_channel_argmax": [c_void_p, c_int, c_int, c_int, c_int64, c_void_p, c_void_p],
 }
 
 _lib = None

@@ -38,6 +38,18 @@ void set_error(const char* fmt, ...);
     }                                                                        \
   } while (0)
 
+// switch over the label dtypes of tio_dtype: F(T) for the element type T
+#define TIO_LABEL_DISPATCH(dtype, name, F)                          \
+  switch (dtype) {                                                  \
+    case TIO_F32: F(float); break;                                  \
+    case TIO_U8: F(uint8_t); break;                                 \
+    case TIO_I8: F(int8_t); break;                                  \
+    case TIO_I16: F(int16_t); break;                                \
+    case TIO_I32: F(int32_t); break;                                \
+    case TIO_I64: F(int64_t); break;                                \
+    default: TIO_CHECK_ARG(false, name ": unknown dtype %d", dtype); \
+  }
+
 // SM count of the current device (132 on an H100 SXM, 114 on an H100 PCIe), read once per
 // device: the grid caps scale with it
 int num_sms();

@@ -19,6 +19,7 @@
 #include <curand_kernel.h>
 
 #include "common.cuh"
+#include "label_lookup.cuh"
 
 namespace tio {
 
@@ -28,39 +29,6 @@ constexpr int kThreads = 256;
 constexpr int kItersPerBlock = 8;  // grid-stride iterations per block: amortises the table load
 constexpr int kMaxLabels = 2048;
 constexpr unsigned long long kNotDrawn = ~0ull;
-
-// `label == int(l)`: integer maps compare exactly; an fp32 map compares in fp32, and since every
-// l came from int() of a voxel value it is exactly representable, so only integral values match.
-template <typename T>
-__device__ __forceinline__ bool label_key(T v, long long& key) {
-  key = (long long)v;
-  return true;
-}
-template <>
-__device__ __forceinline__ bool label_key<float>(float v, long long& key) {
-  if (!(fabsf(v) < 9.2e18f) || truncf(v) != v) return false;
-  key = (long long)v;
-  return true;
-}
-
-template <typename T> constexpr bool kByteLabels = sizeof(T) == 1;
-
-// slot of `v` in the sorted table, or -1
-template <typename T>
-__device__ __forceinline__ int find_slot(T v, const int* lut, const long long* values, int n) {
-  if constexpr (kByteLabels<T>) {
-    return lut[(unsigned)(unsigned char)v];
-  } else {
-    long long key;
-    if (!label_key(v, key)) return -1;
-    int lo = 0, hi = n;
-    while (lo < hi) {
-      const int mid = (lo + hi) >> 1;
-      if (values[mid] < key) lo = mid + 1; else hi = mid;
-    }
-    return (lo < n && values[lo] == key) ? lo : -1;
-  }
-}
 
 template <typename T>
 __global__ void __launch_bounds__(kThreads)
@@ -105,7 +73,7 @@ labels_to_image_kernel(const T* __restrict__ labels, int C, uint32_t vox, uint32
       if (v < N) {
         b[ii] = v / vox;
         const uint32_t r = v - b[ii] * vox;
-        const int slot = find_slot<T>(labels[((size_t)b[ii] * C) * vox + r], lut, values, n);
+        const int slot = find_slot<T, long long>(labels[((size_t)b[ii] * C) * vox + r], lut, values, n);
         if (slot >= 0 && offs[slot] != kNotDrawn) k[ii] = slot;
       }
     }

@@ -592,3 +592,84 @@ def labels_to_image(labels: Tensor, label_values, means, stds, draw=None) -> Ten
                      _stream(labels))
     _count(2 if n else 1)
     return out
+
+
+# ---- label-map utilities (transforms/label/) ----------------------------------------------------
+
+
+def _label_map(src: Tensor, name: str) -> Tensor:
+    _require_cuda(src, name)
+    if src.dtype not in DTYPE_CODES:
+        raise TypeError(f"{name}: unsupported label dtype {src.dtype}")
+    if src.ndim != 5:
+        raise ValueError(f"{name} expects (B, C, I, J, K), got {tuple(src.shape)}")
+    return src.contiguous()
+
+
+def label_lut(src: Tensor, keys: np.ndarray, values: np.ndarray, *, identity: bool) -> Tensor:
+    """``src`` with every element equal to ``keys[i]`` replaced by ``values[i]`` (tables from
+    `tables.label_lut`), and every other element kept (``identity``) or set to 0 — the result of
+    RemapLabels / RemoveLabels (``clone``) or SequentialLabels (``zeros_like``), one pass."""
+    src = _label_map(src, "label_lut")
+    dst = torch.empty_like(src)
+    n = int(keys.shape[0])
+    keys_d, values_d = upload(src.device, keys, values) if n else (None, None)
+    with torch.cuda.device(src.device):
+        _native.call("tio_label_lut", _ptr(src), _ptr(dst), DTYPE_CODES[src.dtype], src.numel(), _ptr(keys_d),
+                     _ptr(values_d), n, int(bool(identity)), _stream(src))
+    _count(2 if n else 1)
+    return dst
+
+
+def label_contour(src: Tensor) -> Tensor:
+    """(B, C, I, J, K) labels -> fp32 1 where the 3x3x3 minimum of float(v) (-1 outside the volume)
+    differs from float(v), else 0 (label/contour.py:52-71)."""
+    src = _label_map(src, "label_contour")
+    dst = torch.empty(src.shape, dtype=torch.float32, device=src.device)
+    if src.numel():
+        b, c, i, j, k = src.shape
+        with torch.cuda.device(src.device):
+            _native.call("tio_label_contour", _ptr(src), DTYPE_CODES[src.dtype], b * c, i, j, k, _ptr(dst),
+                         _stream(src))
+        _count(1)
+    return dst
+
+
+def label_range(src: Tensor) -> tuple[int, int]:
+    """(min, max) of ``long(v)`` over channel 0 of a non-empty (B, C, I, J, K) batch: one small
+    device-to-host read."""
+    src = _label_map(src, "label_range")
+    b, c = src.shape[:2]
+    out = torch.empty(2, dtype=torch.int64, device=src.device)
+    with torch.cuda.device(src.device):
+        _native.call("tio_label_range", _ptr(src), DTYPE_CODES[src.dtype], b, c, src[0, 0].numel(), _ptr(out),
+                     _stream(src))
+    _count(2)
+    lo, hi = out.tolist()
+    return lo, hi
+
+
+def onehot_classes(src: Tensor, num_classes: int) -> Tensor:
+    """(B, C, I, J, K) labels -> (B, num_classes, I, J, K) fp32: channel c is ``long(v) == c`` on
+    channel 0 of the map (label/one_hot.py:64-68).  The caller checks the classes' range first."""
+    src = _label_map(src, "onehot_classes")
+    b, c = src.shape[:2]
+    dst = torch.empty((b, num_classes, *src.shape[2:]), dtype=torch.float32, device=src.device)
+    with torch.cuda.device(src.device):
+        _native.call("tio_onehot_classes", _ptr(src), DTYPE_CODES[src.dtype], b, c, src[0, 0].numel(),
+                     int(num_classes), _ptr(dst), _stream(src))
+    _count(1)
+    return dst
+
+
+def channel_argmax(src: Tensor) -> Tensor:
+    """(B, C, I, J, K) -> (B, 1, I, J, K) fp32 ``argmax(dim=1, keepdim=True).float()``: the first
+    maximum, a NaN counting as the maximum (label/one_hot.py:95-96)."""
+    src = _label_map(src, "channel_argmax")
+    b, c = src.shape[:2]
+    dst = torch.empty((b, 1, *src.shape[2:]), dtype=torch.float32, device=src.device)
+    with torch.cuda.device(src.device):
+        _native.call("tio_channel_argmax", _ptr(src), DTYPE_CODES[src.dtype], b, c, src[0, 0].numel(), _ptr(dst),
+                     _stream(src))
+    _count(1)
+    return dst

@@ -11,6 +11,7 @@ numbers (TorchIO 2.0.0a2, paths relative to src/torchio/transforms/):
 
 from __future__ import annotations
 
+import functools
 import math
 from dataclasses import dataclass
 
@@ -289,3 +290,52 @@ def label_synthesis_tables(means, stds, batch_size: int):
             draw[c] = drawn
             drawn += 1
     return values, draw, mean, std
+
+
+# ---- label-map lookup tables (label/remap_labels.py:50-58, sequential_labels.py:53-61) ----------
+
+_NUMPY_DTYPES = {torch.float32: np.float32, torch.uint8: np.uint8, torch.int8: np.int8,
+                 torch.int16: np.int16, torch.int32: np.int32, torch.int64: np.int64}
+
+
+def label_lut(pairs, dtype: torch.dtype, device) -> tuple[np.ndarray, np.ndarray]:
+    """(keys, values) of what ``for old, new in pairs: data[src == old] = new`` does to a map of
+    ``dtype``, every mask taken on the unmodified ``src``.  keys: ascending stored values that
+    match some ``old`` (int64, or fp32 for fp32 maps); values: the stored ``new`` (numpy ``dtype``).
+
+    The comparison and assignment rules of a Python scalar against a tensor depend on the dtype
+    (u8 == 257 matches 1, fp32 == 2**24 + 1 matches 2**24, u8[mask] = -1 stores 255, i16[mask] =
+    70000 raises), so torch decides each one, on a one-element tensor of ``dtype`` on ``device``:
+    the candidate for ``old`` is ``old`` converted to ``dtype`` and is kept when it compares equal
+    to ``old``; the stored value is what ``t[mask] = new`` leaves (or raises).  A later pair whose
+    candidate equals an earlier one's overrides it, as its index_put runs later."""
+    pairs = [(old, new) for old, new in pairs]
+    return _label_lut(tuple((type(o), o, type(n), n) for o, n in pairs), dtype, torch.device(device))
+
+
+@functools.lru_cache(maxsize=256)
+def _label_lut(items, dtype, device):
+    mask = torch.ones(1, dtype=torch.bool, device=device)
+    candidates, matches, stored = [], [], []
+    for _, old, _, new in items:
+        source = torch.tensor([old], dtype=torch.float64 if isinstance(old, float) else torch.int64)
+        candidate = source.to(device).to(dtype)
+        candidates.append(candidate)
+        matches.append(candidate == old)
+        t = torch.zeros(1, dtype=dtype, device=device)
+        t[mask] = new
+        stored.append(t)
+    if not items:
+        key_dtype = np.float32 if dtype == torch.float32 else np.int64
+        return np.zeros(0, dtype=key_dtype), np.zeros(0, dtype=_NUMPY_DTYPES[dtype])
+    candidates = torch.cat(candidates).tolist()
+    matches = torch.cat(matches).tolist()
+    stored = torch.cat(stored).cpu().numpy()
+    table = {}
+    for candidate, match, value in zip(candidates, matches, stored):
+        if match:
+            table[candidate + 0.0 if dtype == torch.float32 else candidate] = value  # -0.0 -> +0.0
+    keys = sorted(table)
+    key_dtype = np.float32 if dtype == torch.float32 else np.int64
+    return (np.asarray(keys, dtype=key_dtype),
+            np.asarray([table[k] for k in keys], dtype=_NUMPY_DTYPES[dtype]).reshape(len(keys)))
