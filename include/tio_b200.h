@@ -39,7 +39,11 @@ enum tio_dtype {
   TIO_I8 = 2,
   TIO_I16 = 3,
   TIO_I32 = 4,
-  TIO_I64 = 5
+  TIO_I64 = 5,
+  /* images accepted by tio_interpolate / tio_axis_resample only */
+  TIO_F16 = 6,
+  TIO_BF16 = 7,
+  TIO_F64 = 8
 };
 
 enum tio_interp { TIO_NEAREST = 0, TIO_LINEAR = 1, TIO_LABEL_PV = 2 };
@@ -336,6 +340,35 @@ int tio_label_range(const void* src, int dtype, int B, int C, int64_t vox, int64
                     void* stream);
 int tio_channel_argmax(const void* src, int dtype, int B, int C, int64_t vox, float* dst,
                        void* stream);
+
+/*
+ * Resolution changes (spatial/resize.py, spatial/anisotropy.py of the reference), one pass each on
+ * the data's fp32 image: every tap is converted to fp32 and the result back to `dtype` as
+ * `data.float()` ... `.to(dtype)` do.  `dtype` is any tio_dtype code (TIO_F16 / TIO_BF16 / TIO_F64
+ * included); src and dst do not overlap.
+ *
+ * tio_interpolate: dst (volumes, OI, OJ, OK) from src (volumes, I, J, K), ATen's CUDA
+ * upsample_trilinear3d (align_corners=True, `linear` = 1) or upsample_nearest3d (`linear` = 0).
+ *   idx  [2*(OI+OJ+OK)] int32 device: per axis (I, then J, then K) the lower source index of each
+ *        output index, then the upper one (nearest: the upper half is not read)
+ *   lam  [2*(OI+OJ+OK)] fp32 device: per axis the lower weight, then the upper one (NULL: nearest)
+ * out = t0*(h0*(w0*x000 + w1*x001) + h1*(w0*x010 + w1*x011)) + t1*(...), each `a*x + b*y` rounded
+ * as fma(a, x, rn(b*y)), every tap read.  Replaces F.interpolate of Resize.apply_transform
+ * (resize.py:71-76) and, with the nearest-down map composed into `idx`, the two F.interpolate of
+ * _simulate_anisotropy (anisotropy.py:353-392).
+ *
+ * tio_axis_resample: dst (B, C, I, J, K) from src along one axis per batch element, Anisotropy's
+ * per-instance path (_simulate_anisotropy_per_instance and its helpers, anisotropy.py:132-350).
+ *   axis [B] int32 device: 0, 1 or 2, or -1 for an element copied bit for bit (factor <= 1)
+ *   lo, hi [B*L] int32, w [B*L] fp32 device, L >= max(I, J, K): for element b and output index o
+ *        along its axis, the source indices and weight; nearest (`linear` = 0) reads lo only
+ *        (hi, w may be NULL); linear is lo*(1 - w) + hi*w in four rounded fp32 ops
+ */
+int tio_interpolate(const void* src, void* dst, int dtype, int volumes, int I, int J, int K, int OI,
+                    int OJ, int OK, const int32_t* idx, const float* lam, int linear, void* stream);
+int tio_axis_resample(const void* src, void* dst, int dtype, int B, int C, int I, int J, int K,
+                      const int32_t* axis, const int32_t* lo, const int32_t* hi, const float* w, int L,
+                      int linear, void* stream);
 
 #ifdef __cplusplus
 }

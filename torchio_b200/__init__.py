@@ -3,7 +3,8 @@
 Drop-in for the reference's spatial + intensity augmentation chain
 (`Affine`, `ElasticDeformation`, `Spatial`, `LabelsToImage`, `BiasField`, `Blur`,
 `Noise`, `Gamma`, `Compose`), the label-map utilities (`RemapLabels`, `RemoveLabels`,
-`SequentialLabels`, `OneHot`, `Contour`) and its patch path (`UniformSampler`, `Queue`,
+`SequentialLabels`, `OneHot`, `Contour`), the resolution changes (`Anisotropy`,
+`Resize`) and its patch path (`UniformSampler`, `Queue`,
 `SubjectsLoader`) on tensor-backed `Subject` / `SubjectsBatch` data.  The
 tensor math runs in hand-written sm_90a (H100) CUDA kernels exposed through the C-ABI
 of ``include/tio_b200.h``; see DESIGN.md and INTEGRATION.md.
@@ -16,9 +17,9 @@ from .params import Choice
 from .patches import (GridSampler, ImagesLoader, LabelSampler, PatchLocation, PatchSampler, Queue,
                       StudiesLoader, SubjectsLoader, UniformSampler, WeightedSampler, collate_images, collate_studies,
                       collate_subjects)
-from .transforms import (Affine, AppliedTransform, BiasField, Blur, Compose, Contour, Crop, CropOrPad,
+from .transforms import (Affine, Anisotropy, AppliedTransform, BiasField, Blur, Compose, Contour, Crop, CropOrPad,
                          ElasticDeformation, Flip, Gamma, IntensityTransform, LabelsToImage, Noise, Normalize, OneHot, Pad,
-                         RemapLabels, RemoveLabels, Resample, RescaleIntensity, SequentialLabels, Spatial,
+                         RemapLabels, RemoveLabels, Resample, RescaleIntensity, Resize, SequentialLabels, Spatial,
                          SpatialTransform, Standardize, Transform,
                          apply_inverse_transform, execution_device, get_inverse_transform,
                          set_execution_device)
@@ -26,10 +27,10 @@ from .transforms import (Affine, AppliedTransform, BiasField, Blur, Compose, Con
 __version__ = "0.1.0"
 
 __all__ = [
-    "Affine", "AffineMatrix", "AppliedTransform", "BiasField", "Blur", "Choice", "Compose", "Contour", "Crop", "CropOrPad",
+    "Affine", "AffineMatrix", "Anisotropy", "AppliedTransform", "BiasField", "Blur", "Choice", "Compose", "Contour", "Crop", "CropOrPad",
     "ElasticDeformation", "Flip", "Gamma", "GridSampler", "Image", "ImagesBatch", "ImagesLoader", "IntensityTransform",
     "LabelMap", "LabelSampler", "LabelsToImage", "Noise", "Normalize", "OneHot", "Pad", "PatchLocation", "PatchSampler", "Queue", "RemapLabels", "RemoveLabels",
-    "Resample", "RescaleIntensity", "ScalarImage", "SequentialLabels", "Spatial",
+    "Resample", "RescaleIntensity", "Resize", "ScalarImage", "SequentialLabels", "Spatial",
     "SpatialTransform", "Standardize", "StudiesBatch", "StudiesLoader", "Subject", "SubjectsBatch",
     "SubjectsLoader", "Transform", "UniformSampler", "WeightedSampler", "apply_inverse_transform", "collate_images",
     "collate_studies", "collate_subjects", "exact_coords_default", "execution_device", "get_inverse_transform",

@@ -51,6 +51,10 @@ _SIGNATURES = {
     "tio_onehot_classes": [c_void_p, c_int, c_int, c_int, c_int64, c_int, c_void_p, c_void_p],
     "tio_label_range": [c_void_p, c_int, c_int, c_int, c_int64, c_void_p, c_void_p],
     "tio_channel_argmax": [c_void_p, c_int, c_int, c_int, c_int64, c_void_p, c_void_p],
+    "tio_interpolate": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p,
+                        c_void_p, c_int, c_void_p],
+    "tio_axis_resample": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                          c_void_p, c_void_p, c_int, c_int, c_void_p],
 }
 
 _lib = None

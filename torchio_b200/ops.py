@@ -673,3 +673,57 @@ def channel_argmax(src: Tensor) -> Tensor:
                      _stream(src))
     _count(1)
     return dst
+
+
+# ---- resolution changes (spatial/resize.py, spatial/anisotropy.py) ------------------------------
+
+# every label dtype, and fp16 / bf16 / fp64 images, which the kernels compute in fp32 and cast back
+# as the reference's data.float() ... .to(dtype) do (tio_dtype TIO_F16 / TIO_BF16 / TIO_F64)
+RESOLUTION_DTYPE_CODES = {**DTYPE_CODES, torch.float16: 6, torch.bfloat16: 7, torch.float64: 8}
+
+
+def _volume_batch(src: Tensor, name: str) -> Tensor:
+    _require_cuda(src, name)
+    if src.dtype not in RESOLUTION_DTYPE_CODES:
+        raise TypeError(f"{name}: unsupported dtype {src.dtype}")
+    if src.ndim != 5:
+        raise ValueError(f"{name} expects (B, C, I, J, K), got {tuple(src.shape)}")
+    return src.contiguous()
+
+
+def interpolate(src: Tensor, out_shape, idx: np.ndarray, lam: np.ndarray | None) -> Tensor:
+    """(B, C, I, J, K) -> (B, C, *out_shape) of src's dtype: ATen's CUDA trilinear
+    (align_corners=True; ``lam`` given) or nearest resize of ``src.float()``, cast back, from the
+    per-axis tables of `tables.resize_tables` / `tables.anisotropy_shared_tables`, one pass."""
+    src = _volume_batch(src, "interpolate")
+    b, c, i, j, k = src.shape
+    oi, oj, ok = (int(s) for s in out_shape)
+    dst = torch.empty((b, c, oi, oj, ok), dtype=src.dtype, device=src.device)
+    if src.numel() and dst.numel():
+        idx_d, lam_d = upload(src.device, idx, lam)
+        with torch.cuda.device(src.device):
+            _native.call("tio_interpolate", _ptr(src), _ptr(dst), RESOLUTION_DTYPE_CODES[src.dtype], b * c, i, j, k, oi, oj,
+                         ok, _ptr(idx_d), _ptr(lam_d), int(lam is not None), _stream(src))
+        _count(1)
+    return dst
+
+
+def axis_resample(src: Tensor, axis: np.ndarray, lo: np.ndarray, hi: np.ndarray, w: np.ndarray, *,
+                  linear: bool) -> Tensor:
+    """Anisotropy's per-instance degradation of a (B, C, I, J, K) batch, one pass: element b is
+    resampled along ``axis[b]`` from the (lo, hi, w) rows of `tables.anisotropy_instance_tables`
+    (nearest: lo only), or copied when ``axis[b]`` is -1 (anisotropy.py:132-214)."""
+    src = _volume_batch(src, "axis_resample")
+    b, c, i, j, k = src.shape
+    dst = torch.empty_like(src)
+    if src.numel():
+        if linear:
+            axis_d, lo_d, hi_d, w_d = upload(src.device, axis, lo, hi, w)
+        else:
+            (axis_d, lo_d), hi_d, w_d = upload(src.device, axis, lo), None, None
+        with torch.cuda.device(src.device):
+            _native.call("tio_axis_resample", _ptr(src), _ptr(dst), RESOLUTION_DTYPE_CODES[src.dtype], b, c, i, j, k,
+                         _ptr(axis_d), _ptr(lo_d), _ptr(hi_d), _ptr(w_d), int(lo.shape[1]), int(bool(linear)),
+                         _stream(src))
+        _count(1)
+    return dst

@@ -339,3 +339,125 @@ def _label_lut(items, dtype, device):
     key_dtype = np.float32 if dtype == torch.float32 else np.int64
     return (np.asarray(keys, dtype=key_dtype),
             np.asarray([table[k] for k in keys], dtype=_NUMPY_DTYPES[dtype]).reshape(len(keys)))
+
+
+# ---- Resize / Anisotropy index tables (spatial/resize.py, spatial/anisotropy.py) ---------------
+#
+# ATen's CUDA upsample (ATen/native/cuda/UpSample.cuh, restated in fp32 with numpy's
+# round-to-nearest scalar ops):
+#   linear, align_corners=True: scale = float(in - 1) / float(out - 1) (0 when out == 1),
+#     pos = scale * float(o), i0 = int(pos), i1 = i0 + (i0 < in - 1), l1 = pos - float(i0), l0 = 1 - l1
+#   nearest: scale = float(in) / float(out), i = min(floorf(float(o) * scale), in - 1)
+
+
+@functools.lru_cache(maxsize=1024)
+def aten_linear_axis(n_in: int, n_out: int) -> tuple[np.ndarray, np.ndarray, np.ndarray, np.ndarray]:
+    """(i0, i1, l0, l1) of ATen's align_corners=True linear upsample of one axis, n_in -> n_out."""
+    scale = np.float32(n_in - 1) / np.float32(n_out - 1) if n_out > 1 else np.float32(0.0)
+    pos = np.arange(n_out, dtype=np.float32) * scale
+    i0 = pos.astype(np.int64)
+    i1 = i0 + (i0 < n_in - 1)
+    l1 = pos - i0.astype(np.float32)
+    l0 = np.float32(1.0) - l1
+    return i0, i1, l0, l1
+
+
+@functools.lru_cache(maxsize=1024)
+def aten_nearest_axis(n_in: int, n_out: int) -> np.ndarray:
+    """Source index of each output index of ATen's nearest resize of one axis, n_in -> n_out."""
+    scale = np.float32(n_in) / np.float32(n_out)
+    pos = np.arange(n_out, dtype=np.float32) * scale
+    return np.minimum(np.floor(pos).astype(np.int64), n_in - 1)
+
+
+def _pack_axes(axes) -> tuple[np.ndarray, np.ndarray | None]:
+    """[(i0, i1, l0, l1) or i0 per axis] -> the (idx, lam) tables of tio_interpolate."""
+    if all(isinstance(a, np.ndarray) for a in axes):
+        idx = np.concatenate([np.concatenate([a, a]) for a in axes]).astype(np.int32)
+        return idx, None
+    idx = np.concatenate([np.concatenate([a[0], a[1]]) for a in axes]).astype(np.int32)
+    lam = np.concatenate([np.concatenate([a[2], a[3]]) for a in axes]).astype(np.float32)
+    return idx, lam
+
+
+def resize_tables(in_shape, out_shape, linear: bool) -> tuple[np.ndarray, np.ndarray | None]:
+    """(idx, lam) of ``F.interpolate(size=out_shape, mode="trilinear", align_corners=True)``
+    (``linear``) or ``mode="nearest"`` on CUDA; lam is None for a nearest pass.  ATen's trilinear
+    copies when the shapes are equal, which the identity nearest tables reproduce."""
+    in_shape, out_shape = tuple(int(s) for s in in_shape), tuple(int(s) for s in out_shape)
+    if linear and in_shape != out_shape:
+        return _pack_axes([aten_linear_axis(i, o) for i, o in zip(in_shape, out_shape)])
+    return _pack_axes([aten_nearest_axis(i, o) for i, o in zip(in_shape, out_shape)])
+
+
+def anisotropy_shared_tables(shape, axis: int, factor: float, linear: bool):
+    """(idx, lam) of _simulate_anisotropy (anisotropy.py:353-392) as ONE tio_interpolate pass:
+    nearest down to D = max(1, round(L / factor)) along ``axis``, then trilinear
+    (align_corners=True) or nearest back to L.  The up table's source indices along ``axis`` are
+    composed with the down map; the other axes keep their size in both passes, so their up tables
+    are ATen's L -> L ones (trilinear: weight 1 on the voxel, 0 on its neighbour, both read).
+    D == L makes the trilinear pass a copy in ATen."""
+    shape = [int(s) for s in shape]
+    length = shape[axis]
+    down = max(1, round(length / factor))
+    down_map = aten_nearest_axis(length, down)
+    axis = range(3)[axis]
+    if linear and down != length:
+        axes = [aten_linear_axis(n, n) for n in shape]
+        i0, i1, l0, l1 = aten_linear_axis(down, length)
+        axes[axis] = (down_map[i0], down_map[i1], l0, l1)
+    else:
+        axes = [aten_nearest_axis(n, n) for n in shape]
+        axes[axis] = down_map[aten_nearest_axis(down, length)]
+    return _pack_axes(axes)
+
+
+@functools.lru_cache(maxsize=1024)
+def _instance_axis(length: int, down: int, linear: bool):
+    """(lo, hi, w) source indices along the axis of one element (anisotropy.py:238-331), as the
+    reference computes them on a CUDA batch."""
+    def source(lowres):  # _downsample_source_indices: floor(m * L / D) in int64, clamped
+        return np.minimum(lowres * length // down, length - 1)
+
+    if not linear:  # _nearest_source_indices
+        lo = source(np.arange(length, dtype=np.int64) * down // length)
+        return lo, lo, np.zeros(length, dtype=np.float32)
+    if length == 1:
+        pos = np.zeros(1, dtype=np.float32)
+    else:
+        # `(D - 1.0) / (length - 1)` on a CUDA tensor: ATen divides by a Python scalar as a multiply
+        # by its fp32 reciprocal (div_true_kernel_cuda), which the CPU's true division does not
+        scale = (np.float32(down) - np.float32(1.0)) * (np.float32(1.0) / np.float32(length - 1))
+        pos = np.arange(length, dtype=np.float32) * scale
+    lower = np.floor(pos).astype(np.int64)
+    upper = np.minimum(lower + 1, down - 1)
+    return source(lower), source(upper), pos - lower.astype(np.float32)
+
+
+def anisotropy_down_size(length: int, factor: float) -> int:
+    """``torch.round(length / factors)`` of _downsample_sizes (anisotropy.py:219-235), at least 1.
+    ``int / Tensor`` is ``Tensor.__rtruediv__``, which torch runs as ``reciprocal() * int`` in
+    float64, not as a true division: the two round to different sizes near .5 (L = 33, factor 4.4:
+    8 here, 7 by true division).  Half to even, as torch.round."""
+    return max(1, int(np.round(np.float64(length) * (np.float64(1.0) / np.float64(factor)))))
+
+
+def anisotropy_instance_tables(shape, axes, factors, linear: bool):
+    """(axis [B] int32, lo, hi [B, L] int32, w [B, L] fp32) of
+    _simulate_anisotropy_per_instance for tio_axis_resample, L = max(shape); an element with
+    factor <= 1 gets axis -1 (copied).  The caller has checked the active axes are 0, 1 or 2."""
+    shape = [int(s) for s in shape]
+    width = max(shape)
+    n = len(axes)
+    axis = np.full(n, -1, dtype=np.int32)
+    lo = np.zeros((n, width), dtype=np.int32)
+    hi = np.zeros((n, width), dtype=np.int32)
+    w = np.zeros((n, width), dtype=np.float32)
+    for b, (a, f) in enumerate(zip(axes, factors)):
+        if not f > 1.0:
+            continue
+        length = shape[a]
+        rows = _instance_axis(length, anisotropy_down_size(length, f), linear)
+        axis[b] = a
+        lo[b, :length], hi[b, :length], w[b, :length] = rows
+    return axis, lo, hi, w
