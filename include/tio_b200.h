@@ -222,8 +222,8 @@ int tio_randn_mt19937(uint64_t seed, uint64_t offset, uint64_t n, float* z,
  *   tio_quantiles  for each of the m <= 2 quantiles q (host doubles in [0,1]): index = q*(count-1),
  *                  lower = floor(index); values[2t], values[2t+1] = the order statistics of rank
  *                  lower and min(lower+1, count-1) (what torch.kthvalue(lower+1 / lower+2) returns),
- *                  weights[t] = index - lower, *count = number of selected values.  Exact (3-level
- *                  radix select over the order-preserving integer image of fp32), three passes.
+ *                  weights[t] = index - lower, *count = number of selected values.  It is
+ *                  tio_quantiles_batched with B = 1 on fp32 values.
  *                  workspace: tio_quantiles_workspace_bytes() device bytes, 16-byte aligned.
  *   tio_rescale    dst = ((clamp(src, lo, hi) - sub[b]) / div[b]) * mul[b] + add[b] over (B, per_elem),
  *                  each step rounded to fp32 like the reference's separate elementwise ops
@@ -239,6 +239,39 @@ int tio_quantiles(const float* src, const uint8_t* mask, int64_t n, const double
 int tio_rescale(const float* src, float* dst, int B, int64_t per_elem, float lo, float hi,
                 const float* sub, const float* div, const float* mul, const float* add,
                 const uint8_t* keep, int flags, void* stream);
+
+/*
+ * Batched exact quantiles and histogram standardization
+ * (transforms/intensity/histogram_standardization.py:216-303 of the reference, which copies every
+ * element to the host for np.percentile and maps it with ~12 torch ops).
+ *
+ * tio_quantiles_batched: the tio_quantiles statistics for each of B elements of per_elem values
+ *   (src (B, per_elem) of tio_dtype `dtype`, each value taken as `.float()` gives it; mask
+ *   (B, per_elem) or NULL) and m >= 1 quantiles q_host[m] (host doubles in [0, 1]):
+ *   values[B][2m] fp32, weights[B][m] fp64, count[B] fp64, has_nan[B] (NULL: not written) = 1 when
+ *   a selected value is NaN.  Exact: a 3-level radix select over the order-preserving integer image
+ *   of fp32, one launch per level for the whole batch; ranks with a common key prefix share a
+ *   histogram; 13 quantiles per round over levels 1 and 2, more in further rounds.  No host sync.
+ *   workspace: tio_quantiles_batched_workspace_bytes(B, m) device bytes, 16-byte aligned.
+ *   Replaces np.percentile(flat.cpu().numpy(), ...) (histogram_standardization.py:279) and the
+ *   per-image np.percentile of compute_histogram_landmarks (:100-108).
+ * tio_histogram_tables: per element, np.percentile's linear value of each quantile from values /
+ *   weights (d = b - a in fp32, the rest fp64, NaN when has_nan[b]), then the fp32 tables of
+ *   histogram_standardization.py:283-300 for landmarks[m] (device fp32):
+ *   tables[B][3(m-1)] = {slopes[m-1], intercepts[m-1], edges[m-2]}.
+ * tio_histogram_map: dst[b] = slopes[bin] * x + intercepts[bin] (two roundings), bin =
+ *   torch.bucketize(x, edges, right=False), x = src[b] as fp32, stored as torch's CUDA cast to
+ *   `dtype` does; src == dst allowed (histogram_standardization.py:302-303 and the in-place
+ *   `img_batch.data[i] = ...` of :216-227).
+ */
+size_t tio_quantiles_batched_workspace_bytes(int B, int m);
+int tio_quantiles_batched(const void* src, int dtype, const uint8_t* mask, int B, int64_t per_elem,
+                          const double* q_host, int m, float* values, double* weights, double* count,
+                          uint8_t* has_nan, void* workspace, size_t workspace_bytes, void* stream);
+int tio_histogram_tables(const float* values, const double* weights, const uint8_t* has_nan,
+                         const float* landmarks, int B, int m, float* tables, void* stream);
+int tio_histogram_map(const void* src, void* dst, int dtype, int B, int64_t per_elem,
+                      const float* tables, int m, void* stream);
 
 /*
  * Intensity chain: what Compose([BiasField, Blur, Noise, Gamma]) computes, in

@@ -4,7 +4,8 @@ Drop-in for the reference's spatial + intensity augmentation chain
 (`Affine`, `ElasticDeformation`, `Spatial`, `LabelsToImage`, `BiasField`, `Blur`,
 `Noise`, `Gamma`, `Compose`), the label-map utilities (`RemapLabels`, `RemoveLabels`,
 `SequentialLabels`, `OneHot`, `Contour`), the resolution changes (`Anisotropy`,
-`Resize`) and its patch path (`UniformSampler`, `Queue`,
+`Resize`), histogram standardization (`HistogramStandardization`,
+`ZNormalization`) and its patch path (`UniformSampler`, `Queue`,
 `SubjectsLoader`) on tensor-backed `Subject` / `SubjectsBatch` data.  The
 tensor math runs in hand-written sm_90a (H100) CUDA kernels exposed through the C-ABI
 of ``include/tio_b200.h``; see DESIGN.md and INTEGRATION.md.
@@ -18,9 +19,9 @@ from .patches import (GridSampler, ImagesLoader, LabelSampler, PatchLocation, Pa
                       StudiesLoader, SubjectsLoader, UniformSampler, WeightedSampler, collate_images, collate_studies,
                       collate_subjects)
 from .transforms import (Affine, Anisotropy, AppliedTransform, BiasField, Blur, Compose, Contour, Crop, CropOrPad,
-                         ElasticDeformation, Flip, Gamma, IntensityTransform, LabelsToImage, Noise, Normalize, OneHot, Pad,
+                         ElasticDeformation, Flip, Gamma, HistogramStandardization, IntensityTransform, LabelsToImage, Noise, Normalize, OneHot, Pad,
                          RemapLabels, RemoveLabels, Resample, RescaleIntensity, Resize, SequentialLabels, Spatial,
-                         SpatialTransform, Standardize, Transform,
+                         SpatialTransform, Standardize, Transform, ZNormalization,
                          apply_inverse_transform, execution_device, get_inverse_transform,
                          set_execution_device)
 
@@ -28,11 +29,11 @@ __version__ = "0.1.0"
 
 __all__ = [
     "Affine", "AffineMatrix", "Anisotropy", "AppliedTransform", "BiasField", "Blur", "Choice", "Compose", "Contour", "Crop", "CropOrPad",
-    "ElasticDeformation", "Flip", "Gamma", "GridSampler", "Image", "ImagesBatch", "ImagesLoader", "IntensityTransform",
+    "ElasticDeformation", "Flip", "Gamma", "GridSampler", "HistogramStandardization", "Image", "ImagesBatch", "ImagesLoader", "IntensityTransform",
     "LabelMap", "LabelSampler", "LabelsToImage", "Noise", "Normalize", "OneHot", "Pad", "PatchLocation", "PatchSampler", "Queue", "RemapLabels", "RemoveLabels",
     "Resample", "RescaleIntensity", "Resize", "ScalarImage", "SequentialLabels", "Spatial",
     "SpatialTransform", "Standardize", "StudiesBatch", "StudiesLoader", "Subject", "SubjectsBatch",
-    "SubjectsLoader", "Transform", "UniformSampler", "WeightedSampler", "apply_inverse_transform", "collate_images",
+    "SubjectsLoader", "Transform", "UniformSampler", "WeightedSampler", "ZNormalization", "apply_inverse_transform", "collate_images",
     "collate_studies", "collate_subjects", "exact_coords_default", "execution_device", "get_inverse_transform",
     "set_exact_coords", "set_execution_device",
 ]

@@ -31,6 +31,11 @@ _SIGNATURES = {
     "tio_quantiles_workspace_bytes": [],
     "tio_quantiles": [c_void_p, c_void_p, c_int64, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                       c_size_t, c_void_p],
+    "tio_quantiles_batched_workspace_bytes": [c_int, c_int],
+    "tio_quantiles_batched": [c_void_p, c_int, c_void_p, c_int, c_int64, c_void_p, c_int, c_void_p, c_void_p,
+                              c_void_p, c_void_p, c_void_p, c_size_t, c_void_p],
+    "tio_histogram_tables": [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p],
+    "tio_histogram_map": [c_void_p, c_void_p, c_int, c_int, c_int64, c_void_p, c_int, c_void_p],
     "tio_rescale": [c_void_p, c_void_p, c_int, c_int64, c_float, c_float, c_void_p, c_void_p, c_void_p, c_void_p,
                     c_void_p, c_int, c_void_p],
     "tio_onehot": [c_void_p, c_int, c_int, c_int64, c_void_p, c_int, c_void_p, c_void_p],

@@ -21,7 +21,7 @@ SOURCES = ["error.cu", "resample.cu", "resample_tile.cu", "resample_fast.cu", "u
            "mt19937_jump.cpp", "mt19937.cu", "patches.cu", "stats.cu", "labels.cu", "labels_to_image.cu",
            "label_maps.cu", "interpolate.cu"]
 HEADERS = [HERE / "common.cuh", HERE / "resample_common.cuh", HERE / "resample_tile.cuh", HERE / "tma.cuh",
-           HERE / "mt19937_layout.h", HERE / "label_lookup.cuh",
+           HERE / "mt19937_layout.h", HERE / "label_lookup.cuh", HERE / "image_dtype.cuh",
            ROOT / "include" / "tio_b200.h",
            Path(__file__).resolve()]  # the flags below: objects built for another architecture are rebuilt
 OBJ = HERE / "_obj"

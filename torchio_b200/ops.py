@@ -393,9 +393,69 @@ def quantile_neighbours(values: Tensor, qs, mask: Tensor | None = None):
     with torch.cuda.device(dev):
         _native.call("tio_quantiles", _ptr(values), _ptr(m8), values.numel(), qs.ctypes.data, m, _ptr(vals),
                      _ptr(out), out[m:].data_ptr(), _ptr(ws), ws_bytes, _stream(values))
-    _count(8)
+    _count(7)
     host = out.tolist()
     return vals.tolist(), host[:m], int(host[m])
+
+
+def quantiles_batched(values: Tensor, qs, mask: Tensor | None = None):
+    """`quantile_neighbours` for every element of a (B, ...) CUDA tensor of any image dtype (values
+    taken as ``.float()`` gives them), with any number of quantiles, left on the device: returns
+    (values (B, 2m) fp32, weights (B, m) fp64, count (B,) fp64, has_nan (B,) uint8) without a
+    host sync (histogram_standardization.py:100-108,279)."""
+    _require_cuda(values, "quantiles_batched")
+    if values.dtype not in RESOLUTION_DTYPE_CODES:
+        raise TypeError(f"quantiles_batched: unsupported dtype {values.dtype}")
+    values = values.contiguous()
+    b = values.shape[0]
+    per_elem = values[0].numel()
+    m8 = None if mask is None else mask.expand_as(values).contiguous().to(torch.uint8)
+    qs = np.ascontiguousarray(np.asarray(qs, dtype=np.float64).reshape(-1))
+    m = int(qs.shape[0])
+    dev = values.device
+    vals = torch.empty((b, 2 * m), dtype=torch.float32, device=dev)
+    weights = torch.empty((b, m), dtype=torch.float64, device=dev)
+    count = torch.empty(b, dtype=torch.float64, device=dev)
+    has_nan = torch.empty(b, dtype=torch.uint8, device=dev)
+    ws_bytes = _native.lib().tio_quantiles_batched_workspace_bytes(b, m)
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        _native.call("tio_quantiles_batched", _ptr(values), RESOLUTION_DTYPE_CODES[values.dtype], _ptr(m8), b,
+                     per_elem, qs.ctypes.data, m, _ptr(vals), _ptr(weights), _ptr(count), _ptr(has_nan), _ptr(ws),
+                     ws_bytes, _stream(values))
+    _count(2 + 5 * ((m + 12) // 13))
+    return vals, weights, count, has_nan
+
+
+def histogram_tables(values: Tensor, weights: Tensor, has_nan: Tensor, landmarks: Tensor) -> Tensor:
+    """(B, 3 (m - 1)) fp32 device tables {slopes, intercepts, edges} of
+    _apply_histogram_standardization (histogram_standardization.py:279-300) from the output of
+    `quantiles_batched` and the m fp32 landmarks, built on the device."""
+    b, m = weights.shape
+    landmarks = landmarks.to(device=values.device, dtype=torch.float32).contiguous()
+    tables = torch.empty((b, 3 * (m - 1)), dtype=torch.float32, device=values.device)
+    with torch.cuda.device(values.device):
+        _native.call("tio_histogram_tables", _ptr(values), _ptr(weights), _ptr(has_nan), _ptr(landmarks), b, m,
+                     _ptr(tables), _stream(values))
+    _count(1)
+    return tables
+
+
+def histogram_map(data: Tensor, tables: Tensor, m: int) -> None:
+    """In place: each element of the contiguous (B, ...) CUDA tensor ``data`` through its
+    piecewise-linear map ``slopes[bin] * x + intercepts[bin]``, bin = torch.bucketize(x, edges),
+    computed in fp32 and stored in data's dtype (histogram_standardization.py:302-303)."""
+    _require_cuda(data, "histogram_map")
+    if data.dtype not in RESOLUTION_DTYPE_CODES:
+        raise TypeError(f"histogram_map: unsupported dtype {data.dtype}")
+    if not data.is_contiguous():
+        raise ValueError("histogram_map: data must be contiguous")
+    if data.numel() == 0:
+        return
+    with torch.cuda.device(data.device):
+        _native.call("tio_histogram_map", _ptr(data), _ptr(data), RESOLUTION_DTYPE_CODES[data.dtype], data.shape[0],
+                     data[0].numel(), _ptr(tables), int(m), _stream(data))
+    _count(1)
 
 
 def rescale(src: Tensor, *, lo: float | None = None, hi: float | None = None, sub=None, div=None, mul=None,

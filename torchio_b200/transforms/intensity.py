@@ -645,6 +645,7 @@ class Normalize(IntensityTransform):
 
 
 RescaleIntensity = Normalize  # the reference's backwards-compatible alias (normalize.py:369)
+ZNormalization = Standardize  # the reference's backwards-compatible alias (standardize.py:178)
 
 
 def _value_range(value):
