@@ -179,7 +179,9 @@ int tio_min_sample0(const float* src, int C, int64_t n, float* fill, void* strea
  *             blur.py:179-183 / 292-328 (zero beyond each element's radius,
  *             delta kernel where sigma <= 0)
  *   radius    [3][B] int32: the element's own radius on that axis (0 = skip)
- *   R         table half-width (max radius over the whole table)
+ *   R         table half-width (max radius over the whole table), at most 6143;
+ *             R > 16 runs one launch per blurred axis and then needs `scratch`
+ *             whatever the axes
  *   axes_mask host int, bit a set = axis a is active for at least one element
  *             (lets the library skip whole passes without reading `radius`)
  *   identity  [B] bytes: rows with all sigma <= 0 are copied exactly
@@ -300,7 +302,8 @@ int tio_histogram_map(const void* src, void* dst, int dtype, int B, int64_t per_
  *       (transforms/intensity/gamma.py:88-90)
  *   per-element identity rows (bias_identity[b], all radii 0, keep[b] == 0,
  *   gamma[b] == 1) pass through every stage as bit-exact copies
- *   scratch: B*C*I*J*K floats, required when axes_mask has bit 1 or 2 (J/K)
+ *   scratch: B*C*I*J*K floats, required when axes_mask has bit 1 or 2 (J/K), or
+ *            when R > 16 with blur and bias both active, or more than one axis
  * src, dst, scratch must be distinct when blur is active.
  */
 int tio_intensity_fused(const float* src, float* dst, float* scratch,

@@ -54,14 +54,22 @@ __device__ __forceinline__ void box_muller(uint32_t a, uint32_t b, float& n0, fl
 }
 
 
+// |x|^g = 2^(g*log2|x|) on the SFU (lg2/ex2.approx): ~3e-7 relative for the value ranges
+// of normalised images, far inside the 1e-4 parity tolerance.  Neither flushes subnormals:
+// (1e-40)^0.8 = 1e-32 as torch's pow gives, and a subnormal result is kept.
+__device__ __forceinline__ float abs_pow(float ax, float g) {
+  float l, p;
+  asm("lg2.approx.f32 %0, %1;" : "=f"(l) : "f"(ax));
+  asm("ex2.approx.f32 %0, %1;" : "=f"(p) : "f"(__fmul_rn(g, l)));
+  return p;
+}
+
 __device__ __forceinline__ float signed_pow(float x, float gam) {
   // sign(x) * |x|^gamma (gamma.py:88-90); gamma == 1 -> x exactly (gated rows).
-  // |x|^g = 2^(g*log2|x|) on the SFU (lg2/ex2.approx): ~3e-7 relative for the
-  // value ranges of normalised images, far inside the 1e-4 parity tolerance.
+  // sign(+-0) = 0, so +-0 -> +0 as torch gives.
   if (gam == 1.0f) return x;
   float ax = fabsf(x);
-  float p;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(p) : "f"(gam * __log2f(ax)));
+  float p = abs_pow(ax, gam);
   p = ax == 0.0f ? 0.0f : p;
   return x < 0.0f ? -p : p;
 }
@@ -332,12 +340,11 @@ __device__ __forceinline__ void jconv8(const float* __restrict__ Bw, const int j
     for (int o = 0; o < 8; ++o) acc[o] = __fmaf_rn(tj[F_R + t], win[o + t + RJ], acc[o]);
 }
 
-// sign(x) * |x|^g for g > 0 on the SFU: lg2(0) = -inf -> ex2 = 0, so zero needs no select
+// signed_pow for g > 0, g != 1: lg2(0) = -inf -> ex2 = +0, so zero needs no select, and
+// -0 -> +0 because -0 < 0 is false.  Bit-identical to signed_pow for those g.
 __device__ __forceinline__ float signed_pow_pos(float x, float g) {
-  float l, p;
-  asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(l) : "f"(fabsf(x)));
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(p) : "f"(__fmul_rn(g, l)));
-  return copysignf(p, x);
+  const float p = abs_pow(fabsf(x), g);
+  return x < 0.0f ? -p : p;
 }
 
 template <bool HAS_EPI>
@@ -707,8 +714,9 @@ march_kernel(const float* __restrict__ src, float* __restrict__ dst, int B, int 
 // -------------------------------------------------------------------------
 // pass 1, fast variant for table radius R <= 6 and 16-byte aligned rows: the ring of
 // the last 13 planes lives in registers.  The plane loop is unrolled by 13 so every
-// ring slot is a fixed register: per voxel 13 FMAs, no shared-memory traffic, no
-// modular indexing.  Taps are zero-padded to 13 (smaller radii use the same code).
+// ring slot is a fixed register: no shared-memory traffic, no modular indexing.  Only the
+// element's own 2r+1 taps are accumulated (a CTA-uniform predicate per tap, in the order of
+// every other path): a zero tap would turn a NaN or Inf r+1..6 planes away into NaN.
 //   EPI = this is the only pass (no J/K blur): noise and gamma at the store.
 // -------------------------------------------------------------------------
 constexpr int M6_PF = 8;  // cp.async FIFO depth of march6_kernel (power of two)
@@ -890,6 +898,7 @@ march6_kernel(const float* __restrict__ src, float* __restrict__ dst, int B, int
         float acc[4] = {0.0f, 0.0f, 0.0f, 0.0f};
 #pragma unroll
         for (int t = 0; t < W; ++t) {
+          if (t < F_R - r || t > F_R + r) continue;  // CTA-uniform
           const int sl = (ph + 1 + t) % W;  // position p - 12 + t
 #pragma unroll
           for (int q = 0; q < 4; ++q) acc[q] = __fmaf_rn(tp[t], ring[sl][q], acc[q]);
@@ -898,6 +907,67 @@ march6_kernel(const float* __restrict__ src, float* __restrict__ dst, int B, int
       }
     }
   }
+}
+
+// -------------------------------------------------------------------------
+// one blur axis for tables with R > 16 (sigma > 16/3 voxels), any radius: thread <-> output
+// voxel, clamped (replicate) reads along the axis, the element's 2r+1 taps in shared memory,
+// accumulated from offset -r to +r as every other path does.  Consecutive threads are
+// consecutive k, so every tap read is coalesced; the windows of neighbours overlap in L1/L2.
+//   HAS_EPI = last launch of the chain: noise and gamma at the store.
+// -------------------------------------------------------------------------
+constexpr int WIDE_RMAX = 6143;  // 2R+1 fp32 taps in 48 KiB of shared memory
+
+template <bool HAS_EPI>
+__global__ void __launch_bounds__(256)
+axis_kernel(const float* __restrict__ src, float* __restrict__ dst, int B, int C, int I, int J,
+            int K, int axis, BlurArgs bl, NoiseArgs nz, const float* __restrict__ gamma) {
+  extern __shared__ float taps_s[];  // [2r+1]
+  const int bc = blockIdx.y;
+  const int b = bc / C;
+  const int tid = threadIdx.x;
+  const int64_t n = (int64_t)I * J * K;
+  const int r = bl.radius[axis * B + b];
+  for (int t = tid; t < 2 * r + 1; t += 256)
+    taps_s[t] = bl.taps[((int64_t)axis * B + b) * (2 * bl.R + 1) + bl.R - r + t];
+  __syncthreads();
+  const int64_t e = (int64_t)blockIdx.x * 256 + tid;  // voxel within the (b, c) volume
+  if (e >= n) return;
+  const int L = axis == 0 ? I : (axis == 1 ? J : K);
+  const int64_t s = axis == 0 ? (int64_t)J * K : (axis == 1 ? K : 1);
+  const int pos = (int)((e / s) % L);
+  const float* x = src + (int64_t)bc * n + (e - pos * s);
+  float acc;
+  if (r == 0) {
+    acc = x[pos * s];
+  } else {
+    acc = 0.0f;
+    for (int t = 0; t <= 2 * r; ++t) {
+      const int q = min(max(pos - r + t, 0), L - 1);
+      acc = __fmaf_rn(taps_s[t], __ldg(x + q * s), acc);
+    }
+  }
+  const int64_t flat = (int64_t)bc * n + e;
+  if (HAS_EPI) {
+    if (nz.mode != 0 && (!nz.keep || nz.keep[b])) {
+      const float mu = nz.mean[b], sd = nz.std[b];
+      float z1, z2 = 0.0f;
+      if (nz.mode == 1) {
+        z1 = nz.z[flat];
+        if (nz.rician) z2 = nz.z2[flat];
+      } else {
+        const uint2 key = make_uint2((uint32_t)nz.philox_seed, (uint32_t)(nz.philox_seed >> 32));
+        float unused;
+        uint4 rr = philox4x32_10(make_uint4((uint32_t)flat, (uint32_t)((uint64_t)flat >> 32), 0u, 0x77ffu), key);
+        box_muller(rr.x, rr.y, z1, unused);
+        if (nz.rician) box_muller(rr.z, rr.w, z2, unused);
+      }
+      const float n1 = __fadd_rn(mu, __fmul_rn(sd, z1));
+      acc = nz.rician ? rician(acc, n1, __fadd_rn(mu, __fmul_rn(sd, z2))) : __fadd_rn(acc, n1);
+    }
+    if (gamma) acc = signed_pow(acc, gamma[b]);
+  }
+  dst[flat] = acc;
 }
 
 static inline bool aligned16f(const void* p) { return ((uintptr_t)p & 15) == 0; }
@@ -926,33 +996,12 @@ static int launch_jk(const float* src, float* dst, int B, int C, int I, int J, i
   return 0;
 }
 
-static int fused_impl(const float* src, float* dst, float* scratch, int B, int C, int I, int J,
-                      int K, BiasArgs bi, BlurArgs bl, int axes_mask, NoiseArgs nz,
-                      const float* gamma, cudaStream_t st, const char* who) {
-  TIO_CHECK_ARG(src && dst, "%s: null src/dst", who);
-  TIO_CHECK_ARG(B > 0 && C > 0 && I > 0 && J > 0 && K > 0, "%s: bad shape", who);
-  TIO_CHECK_ARG((int64_t)B * C <= 65535, "%s: B*C must be <= 65535", who);
-  if (!bl.taps) axes_mask = 0;
-  TIO_CHECK_ARG(!bl.taps || (bl.radius && bl.R >= 0 && bl.R <= 16),
-                "%s: blur radius table missing or R=%d > 16 unsupported", who, bl.R);
-  const bool need_jk = (axes_mask & 6) != 0;
-  TIO_CHECK_ARG(!need_jk || (scratch && src != dst && scratch != src && scratch != dst),
-                "%s: blur along J/K needs a scratch buffer and src != dst", who);
-  TIO_CHECK_ARG(!((axes_mask & 1) && src == dst && !need_jk), "%s: blur along I needs src != dst", who);
-  if (bi.coarse) {
-    bi.sc_i = up_scale(bi.si, I); bi.sc_j = up_scale(bi.sj, J); bi.sc_k = up_scale(bi.sk, K);
-    TIO_CHECK_ARG((size_t)bi.si * bi.sj * bi.sk * 4 <= 64 * 1024, "%s: coarse bias grid too large", who);
-  }
-  const bool need_i = (axes_mask & 1) != 0;
-  const bool need_march = !need_jk || need_i || bi.coarse != nullptr;
-  const float* cur = src;
-  if (need_march) {
-    // pass 1: bias + I-conv (+ noise/gamma when it is the only pass)
-    BlurArgs ib = bl;
-    if (!need_i) ib.taps = nullptr;
-    NoiseArgs nz1 = need_jk ? NoiseArgs{} : nz;
-    const float* gamma1 = need_jk ? nullptr : gamma;
-    float* out = need_jk ? scratch : dst;
+// pass 1: bias + I-conv (ib.taps == null: no I-conv) + the noise/gamma epilogue when nz1 / gamma1
+// are set; march6_kernel when the table radius is <= 6 and rows are 16-byte aligned
+static int launch_march(const float* cur, float* out, int B, int C, int I, int J, int K,
+                        const BiasArgs& bi, const BlurArgs& ib, const NoiseArgs& nz1,
+                        const float* gamma1, cudaStream_t st, const char* who) {
+  {
     const bool vec = (K % 4 == 0) && aligned16f(cur) && aligned16f(out) &&
                      (nz1.mode != 1 || (aligned16f(nz1.z) && (!nz1.z2 || aligned16f(nz1.z2))));
     const int V = vec ? 4 : 1;
@@ -986,12 +1035,86 @@ static int fused_impl(const float* src, float* dst, float* scratch, int B, int C
     } else if (vec) { if (bi.coarse) TIO_LAUNCH_MARCH(4, true); else TIO_LAUNCH_MARCH(4, false); }
     else { if (bi.coarse) TIO_LAUNCH_MARCH(1, true); else TIO_LAUNCH_MARCH(1, false); }
 #undef TIO_LAUNCH_MARCH
+  }
+  return 0;
+}
+
+// Tables with R > 16: bias (pass 1 without taps), then one axis_kernel launch per active
+// axis in the order I, K, J of the other paths; the epilogue rides on the last launch.  The
+// launches ping-pong between scratch and dst so that the last one writes dst.
+static int wide_impl(const float* src, float* dst, float* scratch, int B, int C, int I, int J,
+                     int K, const BiasArgs& bi, const BlurArgs& bl, int axes_mask,
+                     const NoiseArgs& nz, const float* gamma, cudaStream_t st, const char* who) {
+  TIO_CHECK_ARG(bl.R <= WIDE_RMAX, "%s: blur radius R=%d > %d unsupported", who, bl.R, WIDE_RMAX);
+  int axes[3], na = 0;
+  for (int a : {0, 2, 1})
+    if (axes_mask & (1 << a)) axes[na++] = a;
+  const int steps = na + (bi.coarse ? 1 : 0);
+  TIO_CHECK_ARG(src != dst && (steps < 2 || (scratch && scratch != src && scratch != dst)),
+                "%s: blur radius R=%d > 16 needs src != dst and a scratch buffer", who, bl.R);
+  const int64_t n = (int64_t)I * J * K;
+  TIO_CHECK_ARG((n + 255) / 256 <= 0x7fffffff, "%s: volume too large", who);
+  const float* cur = src;
+  int left = steps;
+  auto next_out = [&]() { return (--left % 2 == 0) ? dst : scratch; };
+  if (bi.coarse) {
+    BlurArgs none = bl;
+    none.taps = nullptr;
+    float* out = next_out();
+    if (launch_march(cur, out, B, C, I, J, K, bi, none, NoiseArgs{}, nullptr, st, who)) return 1;
+    cur = out;
+  }
+  const size_t smem = (size_t)(2 * bl.R + 1) * sizeof(float);
+  dim3 grid((unsigned)((n + 255) / 256), B * C);
+  for (int s = 0; s < na; ++s) {
+    float* out = next_out();
+    if (s == na - 1 && (nz.mode != 0 || gamma))
+      axis_kernel<true><<<grid, 256, smem, st>>>(cur, out, B, C, I, J, K, axes[s], bl, nz, gamma);
+    else
+      axis_kernel<false><<<grid, 256, smem, st>>>(cur, out, B, C, I, J, K, axes[s], bl, nz, gamma);
+    cur = out;
+  }
+  TIO_CHECK_LAUNCH();
+  return 0;
+}
+
+static int fused_impl(const float* src, float* dst, float* scratch, int B, int C, int I, int J,
+                      int K, BiasArgs bi, BlurArgs bl, int axes_mask, NoiseArgs nz,
+                      const float* gamma, cudaStream_t st, const char* who) {
+  TIO_CHECK_ARG(src && dst, "%s: null src/dst", who);
+  TIO_CHECK_ARG(B > 0 && C > 0 && I > 0 && J > 0 && K > 0, "%s: bad shape", who);
+  TIO_CHECK_ARG((int64_t)B * C <= 65535, "%s: B*C must be <= 65535", who);
+  if (!bl.taps) axes_mask = 0;
+  TIO_CHECK_ARG(!bl.taps || (bl.radius && bl.R >= 0), "%s: blur radius table missing or R=%d < 0", who, bl.R);
+  if (bi.coarse) {
+    bi.sc_i = up_scale(bi.si, I); bi.sc_j = up_scale(bi.sj, J); bi.sc_k = up_scale(bi.sk, K);
+    TIO_CHECK_ARG((size_t)bi.si * bi.sj * bi.sk * 4 <= 64 * 1024, "%s: coarse bias grid too large", who);
+  }
+  if (axes_mask != 0 && bl.R > 16)
+    return wide_impl(src, dst, scratch, B, C, I, J, K, bi, bl, axes_mask, nz, gamma, st, who);
+  const bool need_jk = (axes_mask & 6) != 0;
+  TIO_CHECK_ARG(!need_jk || (scratch && src != dst && scratch != src && scratch != dst),
+                "%s: blur along J/K needs a scratch buffer and src != dst", who);
+  TIO_CHECK_ARG(!((axes_mask & 1) && src == dst && !need_jk), "%s: blur along I needs src != dst", who);
+  const bool need_i = (axes_mask & 1) != 0;
+  const bool need_march = !need_jk || need_i || bi.coarse != nullptr;
+  const float* cur = src;
+  if (need_jk) {
+    // checked before any launch
+    const int64_t tiles = (int64_t)B * C * ((I + A_PLANES - 1) / A_PLANES);
+    TIO_CHECK_ARG(tiles <= 65535, "%s: batch too large for the blur grid", who);
+  }
+  if (need_march) {
+    BlurArgs ib = bl;
+    if (!need_i) ib.taps = nullptr;
+    float* out = need_jk ? scratch : dst;
+    if (launch_march(cur, out, B, C, I, J, K, bi, ib, need_jk ? NoiseArgs{} : nz,
+                     need_jk ? nullptr : gamma, st, who))
+      return 1;
     cur = out;
   }
   if (need_jk) {
     // pass 2: K-conv, J-conv, then noise and gamma at the store
-    const int64_t tiles = (int64_t)B * C * ((I + A_PLANES - 1) / A_PLANES);
-    TIO_CHECK_ARG(tiles <= 65535, "%s: batch too large for the blur grid", who);
     // TMA: 16-byte aligned base and row pitch; coordinates must fit int32
     const bool tma_ok = bl.R <= F_R && (K % 4 == 0) && aligned16f(cur) && (int64_t)B * C * I < (1ll << 31);
     EncodeTiledFn encode = tma_ok ? encode_tiled_fn() : nullptr;

@@ -345,17 +345,24 @@ def blur(src: Tensor, taps: Tensor, radius: Tensor, big_r: int, axes_mask: int,
     src = src.contiguous()
     b, c, i, j, k = src.shape
     dst = torch.empty_like(src)
-    scratch = torch.empty_like(src) if (axes_mask & 6) else None
+    scratch = torch.empty_like(src) if (axes_mask & 6) or big_r > WIDE_R else None
     with torch.cuda.device(src.device):
         _native.call(
             "tio_blur", _ptr(src), _ptr(dst), _ptr(scratch), b, c, i, j, k, _ptr(taps),
             _ptr(radius), int(big_r), int(axes_mask), _ptr(identity), _stream(src),
         )
-    _count(_fused_launches(axes_mask, False))
+    _count(_fused_launches(axes_mask, False, big_r))
     return dst
 
 
-def _fused_launches(axes_mask: int, has_bias: bool) -> int:
+#: Tables with a larger radius run one launch per blurred axis (after the bias pass), through
+#: a scratch buffer whatever the axes.
+WIDE_R = 16
+
+
+def _fused_launches(axes_mask: int, has_bias: bool, big_r: int = 0) -> int:
+    if axes_mask & 7 and big_r > WIDE_R:
+        return bin(axes_mask & 7).count("1") + int(has_bias)
     jk = bool(axes_mask & 6)
     march = (not jk) or bool(axes_mask & 1) or has_bias
     return int(jk) + int(march)
@@ -503,7 +510,7 @@ def intensity_fused(
     src = src.contiguous()
     b, c, i, j, k = src.shape
     dst = torch.empty_like(src)
-    jk = taps is not None and (axes_mask & 6)
+    jk = taps is not None and ((axes_mask & 6) or (axes_mask & 7 and big_r > WIDE_R))
     scratch = torch.empty_like(src) if jk else None
     si = sj = sk = 0
     if coarse is not None:
@@ -517,7 +524,7 @@ def intensity_fused(
             int(philox_seed) & (2**64 - 1), int(noise_mode), int(bool(rician)),
             _ptr(gamma), _stream(src),
         )
-    _count(_fused_launches(axes_mask if taps is not None else 0, coarse is not None))
+    _count(_fused_launches(axes_mask if taps is not None else 0, coarse is not None, big_r))
     return dst
 
 
