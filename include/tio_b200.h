@@ -406,6 +406,52 @@ int tio_axis_resample(const void* src, void* dst, int dtype, int B, int C, int I
                       const int32_t* axis, const int32_t* lo, const int32_t* hi, const float* w, int L,
                       int linear, void* stream);
 
+/*
+ * Clamp, Mask and Swap (intensity/clamp.py, mask.py, swap.py of the reference), one launch each.
+ * Image dtypes are tio_dtype codes, TIO_F16 / TIO_BF16 / TIO_F64 included.
+ *
+ * tio_clamp: dst = torch.clamp(src, min = *lo, max = *hi) over `count` elements.  Replaces
+ * `img_batch.data.clamp(min=out_min, max=out_max)` (clamp.py:53-56).
+ *   lo, hi     host pointers to one value of `dst_dtype` (the bound as torch converts it to the
+ *              result dtype), or NULL for no bound; at least one is given
+ *   dst_dtype  `dtype`, or TIO_F32 for an integer image clamped to a float bound (torch's promotion)
+ * A NaN element stays NaN; with both bounds and either of them NaN every output is that NaN
+ * (ATen's clamp_out).  In place (src == dst) when dst_dtype == dtype.
+ *
+ * tio_mask: torch.where(mask.expand_as(x), x, outside) over x = (B, C, vox).  Replaces
+ * Mask.apply_transform (mask.py:61-97).
+ *   mask        (mask_channels, vox) device, any label dtype (bool as TIO_U8); mask_channels is 1
+ *               (every image channel) or C; the same mask applies to every batch element
+ *   keys        n_keys < 0: a voxel is inside when it is nonzero (`.bool()`); n_keys >= 0: inside
+ *               when it equals one of the ascending device keys (int64, fp32 for fp32 masks; as
+ *               tio_label_lut's), so n_keys = 0 puts every voxel outside
+ *   outside     host pointer to one value of `dst_dtype`
+ *   dst_dtype   == dtype: in place (src NULL or == dst), only the outside voxels are written and
+ *               the image is not read; TIO_F32 for an integer image (promotion by a float
+ *               outside value): dst = inside ? float(src) : outside, src != dst
+ *
+ * tio_swap_patches: Swap's patch exchanges (swap.py:195-364), in place in `data` (B, C, I, J, K) of
+ * `elem_size`-byte elements (1, 2, 4 or 8; the bytes are moved verbatim).
+ *   swaps         host int32 [lists][steps][8]: ai, aj, ak, bi, bj, bk, kind, 0.  kind 0: the two
+ *                 patches do not overlap (checked); 1: they may overlap, the region at b ends up
+ *                 with the old patch at a and the rest of the region at a with the old patch at b;
+ *                 2: no-op.  Every patch must lie inside the volume (checked before any launch).
+ *   lists         1 (one list for every element) or B (element b runs list b)
+ *   swaps_device  device int32 buffer of the same size; the list is copied there on `stream`
+ *   stage         device scratch of B * 2 * C * pi * pj * pk elements, or NULL when no step has
+ *                 kind 1
+ * The steps run in order; each element's list runs on one thread-block cluster (up to 8 CTAs)
+ * with a cluster barrier between steps, all elements in one launch.
+ */
+int tio_clamp(const void* src, void* dst, int dtype, int dst_dtype, int64_t count, const void* lo,
+              const void* hi, void* stream);
+int tio_mask(const void* mask, int mask_dtype, int mask_channels, const void* keys, int n_keys,
+             const void* src, int dtype, void* dst, int dst_dtype, int B, int C, int64_t vox,
+             const void* outside, void* stream);
+int tio_swap_patches(void* data, int elem_size, int B, int C, int I, int J, int K, int pi, int pj,
+                     int pk, const int32_t* swaps, int lists, int steps, int32_t* swaps_device,
+                     void* stage, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -60,6 +60,10 @@ _SIGNATURES = {
                         c_void_p, c_int, c_void_p],
     "tio_axis_resample": [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                           c_void_p, c_void_p, c_int, c_int, c_void_p],
+    "tio_clamp": [c_void_p, c_void_p, c_int, c_int, c_int64, c_void_p, c_void_p, c_void_p],
+    "tio_mask": [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int64,
+                 c_void_p, c_void_p],
+    "tio_swap_patches": [c_void_p] + [c_int] * 9 + [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p],
 }
 
 _lib = None

@@ -794,3 +794,97 @@ def axis_resample(src: Tensor, axis: np.ndarray, lo: np.ndarray, hi: np.ndarray,
                          _stream(src))
         _count(1)
     return dst
+
+
+# ---- Clamp, Mask, Swap (intensity/clamp.py, mask.py, swap.py) ----------------------------------
+
+
+def _scalar_bytes(value: Tensor | None):
+    """(keep-alive array, host address) of a one-element CPU tensor's bytes, or (None, None)."""
+    if value is None:
+        return None, None
+    raw = value.reshape(1).contiguous().view(torch.uint8).numpy()
+    return raw, raw.ctypes.data
+
+
+def clamp(src: Tensor, lo: Tensor | None, hi: Tensor | None) -> Tensor:
+    """``torch.clamp(src, lo, hi)`` in one pass (clamp.py:53-56) into a new tensor of the bounds' dtype:
+    ``lo`` / ``hi`` are one-element CPU tensors holding the bounds as torch converts them to the
+    result dtype (None: no bound), which is src's dtype or fp32 for an integer image."""
+    _require_cuda(src, "clamp")
+    if src.dtype not in RESOLUTION_DTYPE_CODES:
+        raise TypeError(f"clamp: unsupported dtype {src.dtype}")
+    bound = lo if lo is not None else hi
+    if bound is None:
+        raise ValueError("clamp: no bound")
+    src = src.contiguous()
+    dst = torch.empty(src.shape, dtype=bound.dtype, device=src.device)
+    (lo_keep, lo_ptr), (hi_keep, hi_ptr) = _scalar_bytes(lo), _scalar_bytes(hi)
+    with torch.cuda.device(src.device):
+        _native.call("tio_clamp", _ptr(src), _ptr(dst), RESOLUTION_DTYPE_CODES[src.dtype],
+                     RESOLUTION_DTYPE_CODES[dst.dtype], src.numel(), lo_ptr, hi_ptr, _stream(src))
+    _count(1)
+    del lo_keep, hi_keep
+    return dst
+
+
+def mask(data: Tensor, mask: Tensor, keys: np.ndarray | None, outside: Tensor) -> Tensor:
+    """``torch.where(mask.expand_as(data), data, outside)`` (mask.py:61-71) for a (B, C, I, J, K) batch
+    and the (1 or C, I, J, K) mask of one element (bool or a label dtype): inside = nonzero, or equal
+    to one of ``keys`` (`tables.label_lut`'s keys).  ``outside`` is a one-element CPU tensor of the
+    result dtype.  Same dtype: ``data`` is updated in place (only outside voxels are written) and
+    returned; fp32 (an integer image): a new fp32 tensor."""
+    _require_cuda(data, "mask")
+    _require_cuda(mask, "mask")
+    if data.dtype not in RESOLUTION_DTYPE_CODES:
+        raise TypeError(f"mask: unsupported dtype {data.dtype}")
+    if mask.dtype == torch.bool:
+        mask = mask.view(torch.uint8)
+    if mask.dtype not in DTYPE_CODES:
+        raise TypeError(f"mask: unsupported mask dtype {mask.dtype}")
+    if data.ndim != 5 or mask.ndim != 4 or mask.shape[0] not in (1, data.shape[1]) or mask.shape[1:] != data.shape[2:]:
+        raise ValueError(f"mask: a {tuple(mask.shape)} mask for a {tuple(data.shape)} batch")
+    if not data.is_contiguous():
+        raise ValueError("mask: data must be contiguous")
+    mask = mask.contiguous()
+    b, c = data.shape[:2]
+    promote = outside.dtype != data.dtype
+    dst = torch.empty(data.shape, dtype=outside.dtype, device=data.device) if promote else data
+    n = -1 if keys is None else int(keys.shape[0])
+    (keys_d,) = upload(data.device, keys) if n > 0 else (None,)
+    keep, outside_ptr = _scalar_bytes(outside)
+    if data.numel():
+        with torch.cuda.device(data.device):
+            _native.call("tio_mask", _ptr(mask), DTYPE_CODES[mask.dtype], mask.shape[0], _ptr(keys_d), n,
+                         _ptr(data), RESOLUTION_DTYPE_CODES[data.dtype], _ptr(dst), RESOLUTION_DTYPE_CODES[dst.dtype],
+                         b, c, data[0, 0].numel(), outside_ptr, _stream(data))
+        _count(2 if n > 0 else 1)
+    del keep
+    return dst
+
+
+SWAP_EXCHANGE, SWAP_STAGED, SWAP_NOOP = 0, 1, 2
+
+
+def swap_patches(data: Tensor, swaps: np.ndarray, patch_size) -> None:
+    """In place: Swap's ordered patch exchanges (swap.py:195-364) on a contiguous (B, C, I, J, K)
+    CUDA batch.  ``swaps``: int32 (1 or B, steps, 8) rows ``ai, aj, ak, bi, bj, bk, kind, 0`` (kind
+    SWAP_EXCHANGE for a pair that does not overlap, SWAP_STAGED for one that may, SWAP_NOOP), one
+    list for every element or one per element; checked against the volume before any launch."""
+    _require_cuda(data, "swap_patches")
+    if data.ndim != 5 or not data.is_contiguous():
+        raise ValueError(f"swap_patches expects a contiguous (B, C, I, J, K) batch, got {tuple(data.shape)}")
+    swaps = np.ascontiguousarray(swaps, dtype=np.int32)
+    lists, steps = swaps.shape[:2]
+    if steps == 0 or data.numel() == 0:
+        return
+    b, c, i, j, k = data.shape
+    pi, pj, pk = (int(p) for p in patch_size)
+    device_list = torch.empty(swaps.size, dtype=torch.int32, device=data.device)
+    stage = None
+    if bool((swaps[..., 6] == SWAP_STAGED).any()):
+        stage = torch.empty(b * 2 * c * pi * pj * pk * data.element_size(), dtype=torch.uint8, device=data.device)
+    with torch.cuda.device(data.device):
+        _native.call("tio_swap_patches", _ptr(data), data.element_size(), b, c, i, j, k, pi, pj, pk,
+                     swaps.ctypes.data, lists, steps, _ptr(device_list), _ptr(stage), _stream(data))
+    _count(2)

@@ -481,16 +481,22 @@ def _resolve_mask(masking_method, img_batch, batch) -> Tensor | None:
     if callable(masking_method) and not isinstance(masking_method, str):
         return masking_method(img_batch.data[0]).bool()
     if isinstance(masking_method, str):
-        if masking_method not in batch.images:
-            raise KeyError(f'Masking method "{masking_method}" not found in batch images.'
-                           f" Available: {list(batch.images.keys())}")
-        mask_batch = batch.images[masking_method]
-        from ..data import LabelMap
-
-        if not issubclass(mask_batch._image_class, LabelMap):
-            raise TypeError(f'Masking method "{masking_method}" must refer to a LabelMap.')
-        return mask_batch.data[0].bool()
+        return label_map_element0(masking_method, batch).bool()
     raise TypeError(f"masking_method must be None, str, or callable, got {type(masking_method)}")
+
+
+def label_map_element0(key: str, batch) -> Tensor:
+    """Batch element 0 of the `LabelMap` named ``key``, with the reference's errors for a missing key
+    or an image of another class (standardize.py:144-170, mask.py:79-91)."""
+    if key not in batch.images:
+        raise KeyError(f'Masking method "{key}" not found in batch images.'
+                       f" Available: {list(batch.images.keys())}")
+    mask_batch = batch.images[key]
+    from ..data import LabelMap
+
+    if not issubclass(mask_batch._image_class, LabelMap):
+        raise TypeError(f'Masking method "{key}" must refer to a LabelMap.')
+    return mask_batch.data[0]
 
 
 def _sample0(img_batch, mask, warn_empty: str) -> tuple[Tensor, Tensor | None]:
