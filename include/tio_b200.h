@@ -452,6 +452,47 @@ int tio_swap_patches(void* data, int elem_size, int B, int C, int I, int J, int 
                      int pk, const int32_t* swaps, int lists, int steps, int32_t* swaps_device,
                      void* stage, void* stream);
 
+/*
+ * KeepLargestComponent (label/keep_largest.py:63-125 of the reference: per element and label a
+ * compare pass, a host copy, SimpleITK's ConnectedComponent + RelabelComponent, a copy back and an
+ * index_put).  Here every selected label of every element is labelled in one union-find on the
+ * device.  `src` / `data` is B contiguous (I, J, K) volumes of a label dtype, I*J*K < 2^32, B <= 65535.
+ *
+ * Which voxels take part (`mode`), with `keys` [n_keys] on the device:
+ *   0  explicit labels: the value equals a key (keys as tio_label_lut's: ascending, int64, fp32 for
+ *      fp32 maps; an 8-bit map holds at most 256); slot = the key's index
+ *   1  labels=None on U8 / I8 / I16 maps: long(v) != background (when has_background); slot = the
+ *      value (256 or 65536 slots per element)
+ *   2  labels=None on I32 / I64 / F32 maps: long(v) != background, and for fp32 v finite and
+ *      integral (has_background = 0 when no fp32 value equals the background label); slot = the
+ *      index of v in `keys`, the ascending distinct values of the roots (tio_component_roots; int64,
+ *      fp32 for fp32 maps), not needed by tio_components
+ * Two neighbouring voxels that take part are connected when their values compare equal; 26
+ * neighbours when `fully_connected`, else 6.
+ *
+ * tio_components: parent [B * I*J*K] uint32 = for a voxel that takes part, the smallest C-order
+ * index (i*J + j)*K + k within its element of the voxels of its component (the root), else
+ * 0xFFFFFFFF; count [B * I*J*K] uint32 = at a root, the size of its component (0 elsewhere);
+ * flags [B] uint32 = per element bit 0: some voxel takes part, bit 1: a NaN, bit 2: a +-Inf.
+ *
+ * tio_component_roots: values (at least B*vox elements of `dtype`) = the value of every root, in no
+ * particular order; *n_values (device) = how many.
+ *
+ * tio_keep_largest: in place, every voxel that takes part and is not in its (element, slot)'s
+ * largest component (ties: the smallest root) becomes *fill (host pointer to one value of
+ * `dtype`: what `t[mask] = background_label` stores); no other voxel is written.  parent / count
+ * from tio_components on the same data; winner: device scratch of B * slots uint64 (slots =
+ * n_keys, or 256 / 65536 for mode 1).
+ */
+int tio_components(const void* src, int dtype, int B, int I, int J, int K, int mode, const void* keys,
+                   int n_keys, int64_t background, int has_background, int fully_connected,
+                   uint32_t* parent, uint32_t* count, uint32_t* flags, void* stream);
+int tio_component_roots(const void* src, int dtype, int B, int64_t vox, const uint32_t* parent,
+                        void* values, uint32_t* n_values, void* stream);
+int tio_keep_largest(void* data, int dtype, int B, int64_t vox, int mode, const void* keys,
+                     int n_keys, int64_t background, int has_background, const uint32_t* parent,
+                     const uint32_t* count, uint64_t* winner, const void* fill, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

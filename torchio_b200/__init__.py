@@ -3,7 +3,7 @@
 Drop-in for the reference's spatial + intensity augmentation chain
 (`Affine`, `ElasticDeformation`, `Spatial`, `LabelsToImage`, `BiasField`, `Blur`,
 `Noise`, `Gamma`, `Compose`), the label-map utilities (`RemapLabels`, `RemoveLabels`,
-`SequentialLabels`, `OneHot`, `Contour`), the resolution changes (`Anisotropy`,
+`SequentialLabels`, `OneHot`, `Contour`, `KeepLargestComponent`), the resolution changes (`Anisotropy`,
 `Resize`), histogram standardization (`HistogramStandardization`,
 `ZNormalization`), `Clamp`, `Mask`, `Swap` and its patch path (`UniformSampler`, `Queue`,
 `SubjectsLoader`) on tensor-backed `Subject` / `SubjectsBatch` data.  The
@@ -19,7 +19,7 @@ from .patches import (GridSampler, ImagesLoader, LabelSampler, PatchLocation, Pa
                       StudiesLoader, SubjectsLoader, UniformSampler, WeightedSampler, collate_images, collate_studies,
                       collate_subjects)
 from .transforms import (Affine, Anisotropy, AppliedTransform, BiasField, Blur, Clamp, Compose, Contour, Crop, CropOrPad,
-                         ElasticDeformation, Flip, Gamma, HistogramStandardization, IntensityTransform, LabelsToImage, Mask, Noise, Normalize, OneHot, Pad,
+                         ElasticDeformation, Flip, Gamma, HistogramStandardization, IntensityTransform, KeepLargestComponent, LabelsToImage, Mask, Noise, Normalize, OneHot, Pad,
                          RemapLabels, RemoveLabels, Resample, RescaleIntensity, Resize, SequentialLabels, Spatial,
                          SpatialTransform, Swap, Standardize, Transform, ZNormalization,
                          apply_inverse_transform, execution_device, get_inverse_transform,
@@ -30,7 +30,7 @@ __version__ = "0.1.0"
 __all__ = [
     "Affine", "AffineMatrix", "Anisotropy", "AppliedTransform", "BiasField", "Blur", "Choice", "Clamp", "Compose", "Contour", "Crop", "CropOrPad",
     "ElasticDeformation", "Flip", "Gamma", "GridSampler", "HistogramStandardization", "Image", "ImagesBatch", "ImagesLoader", "IntensityTransform",
-    "LabelMap", "LabelSampler", "LabelsToImage", "Mask", "Noise", "Normalize", "OneHot", "Pad", "PatchLocation", "PatchSampler", "Queue", "RemapLabels", "RemoveLabels",
+    "KeepLargestComponent",     "LabelMap", "LabelSampler", "LabelsToImage", "Mask", "Noise", "Normalize", "OneHot", "Pad", "PatchLocation", "PatchSampler", "Queue", "RemapLabels", "RemoveLabels",
     "Resample", "RescaleIntensity", "Resize", "ScalarImage", "SequentialLabels", "Spatial",
     "SpatialTransform", "Standardize", "StudiesBatch", "StudiesLoader", "Subject", "SubjectsBatch",
     "SubjectsLoader", "Swap", "Transform", "UniformSampler", "WeightedSampler", "ZNormalization", "apply_inverse_transform", "collate_images",

@@ -64,6 +64,9 @@ _SIGNATURES = {
     "tio_mask": [c_void_p, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_int64,
                  c_void_p, c_void_p],
     "tio_swap_patches": [c_void_p] + [c_int] * 9 + [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p],
+    "tio_components": [c_void_p] + [c_int] * 6 + [c_void_p, c_int, c_int64, c_int, c_int] + [c_void_p] * 4,
+    "tio_component_roots": [c_void_p, c_int, c_int, c_int64] + [c_void_p] * 4,
+    "tio_keep_largest": [c_void_p, c_int, c_int, c_int64, c_int, c_void_p, c_int, c_int64, c_int] + [c_void_p] * 5,
 }
 
 _lib = None

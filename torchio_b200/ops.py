@@ -888,3 +888,99 @@ def swap_patches(data: Tensor, swaps: np.ndarray, patch_size) -> None:
         _native.call("tio_swap_patches", _ptr(data), data.element_size(), b, c, i, j, k, pi, pj, pk,
                      swaps.ctypes.data, lists, steps, _ptr(device_list), _ptr(stage), _stream(data))
     _count(2)
+
+
+# ---- KeepLargestComponent (label/keep_largest.py) -----------------------------------------------
+
+KEEP_KEYS, KEEP_VALUE, KEEP_SEARCH = 0, 1, 2  # tio_components' modes
+KEEP_PRESENT, KEEP_NAN, KEEP_INF = 1, 2, 4     # its per-element flags
+
+
+def _background_key(background_label, dtype: torch.dtype) -> tuple[int, int]:
+    """(key, has_key) of ``int(v) != background_label`` for labels=None: has_key 0 when no value of a
+    ``dtype`` map can equal the label (outside int64, or not exactly an fp32 value)."""
+    if isinstance(background_label, float) and not background_label.is_integer():
+        return 0, 0
+    key = int(background_label)
+    if not -2**63 <= key < 2**63:
+        return 0, 0
+    if dtype == torch.float32 and int(np.float32(key)) != key:
+        return 0, 0
+    return key, 1
+
+
+def keep_largest(data: Tensor, labels, background_label, fully_connected: bool) -> tuple[Tensor, Tensor]:
+    """In place on a (B, 1, I, J, K) CUDA label batch: within each element and each label, every
+    connected component but the largest (ties: the one whose first voxel in C order comes first) is
+    set to ``background_label`` (label/keep_largest.py:63-125).  ``labels``: the labels to filter
+    (``data == label`` under torch's scalar rules, `tables.label_lut`), or None for every value with
+    ``int(v) != background_label``; ``fully_connected``: 26 neighbours, else 6.
+
+    Returns (data, roots): ``data`` is the input itself when it was contiguous; ``roots`` (B, I, J, K)
+    int32, read as uint32, holds for each voxel that takes part the smallest C-order index of its
+    component within its element, and -1 elsewhere.  Errors the reference raises (NaN / ±Inf with
+    labels=None on fp32 maps, a background label the dtype cannot hold) are raised before anything
+    is written, by the first element in batch order that would raise them."""
+    if data.ndim != 5:
+        raise ValueError(f"keep_largest expects (B, 1, I, J, K), got {tuple(data.shape)}")
+    b, c, i, j, k = (int(s) for s in data.shape)
+    if c != 1:
+        raise ValueError(f"keep_largest expects single-channel label maps, got {c} channels")
+    vox = i * j * k
+    if vox >= 2**32:
+        raise ValueError(f"keep_largest: {vox} voxels per element; component roots are 32-bit (at most 2**32 - 1)")
+    if b > 65535:
+        raise ValueError(f"keep_largest: {b} elements, at most 65535")
+    data = _label_map(data, "keep_largest")
+    dtype, dev = data.dtype, data.device
+    fill, fill_error = None, None
+    try:
+        _, fill = tables.label_lut([(0, background_label)], dtype, dev)  # what t[mask] = label stores
+    except (RuntimeError, ValueError, OverflowError, TypeError) as exc:
+        fill_error = exc
+    key, has_key = _background_key(background_label, dtype)
+    if labels is not None:
+        mode = KEEP_KEYS
+        keys, _ = tables.label_lut([(label, 0) for label in labels], dtype, dev)
+        n = int(keys.shape[0])
+        (keys_d,) = upload(dev, keys) if n else (None,)
+    else:
+        mode = KEEP_VALUE if data.element_size() <= 2 else KEEP_SEARCH
+        keys_d, n = None, 0
+    roots = torch.empty((b, i, j, k), dtype=torch.int32, device=dev)
+    count = torch.empty_like(roots)
+    flags = torch.empty(b, dtype=torch.int32, device=dev)
+    code = DTYPE_CODES[dtype]
+    with torch.cuda.device(dev):
+        _native.call("tio_components", _ptr(data), code, b, i, j, k, mode, _ptr(keys_d), n, key, has_key,
+                     int(bool(fully_connected)), _ptr(roots), _ptr(count), _ptr(flags), _stream(data))
+        _count(3)
+        if mode == KEEP_SEARCH and b * vox:
+            values = torch.empty(b * vox, dtype=dtype, device=dev)
+            n_values = torch.empty(1, dtype=torch.int32, device=dev)
+            _native.call("tio_component_roots", _ptr(data), code, b, vox, _ptr(roots), _ptr(values),
+                         _ptr(n_values), _stream(data))
+            _count(1)
+            found = values[:int(n_values.item())]  # the one read-back: the distinct labels present
+            keys_d = torch.unique(found).to(torch.float32 if dtype == torch.float32 else torch.int64).contiguous()
+            n = int(keys_d.numel())
+            del values
+    if (labels is None and dtype == torch.float32) or fill_error is not None:
+        for bits in flags.tolist():
+            if labels is None and bits & KEEP_INF:
+                raise OverflowError("cannot convert float infinity to integer")
+            if labels is None and bits & KEEP_NAN:
+                raise ValueError("cannot convert float NaN to integer")
+            if fill_error is not None and bits & KEEP_PRESENT:
+                raise fill_error
+    if fill_error is not None or not b * vox or (mode != KEEP_VALUE and n == 0):
+        return data, roots  # nothing takes part
+    slots = n if mode != KEEP_VALUE else (65536 if data.element_size() == 2 else 256)
+    winner = torch.empty(b * slots, dtype=torch.int64, device=dev)
+    keep, fill_ptr = _scalar_bytes(torch.from_numpy(np.ascontiguousarray(fill[:1])))
+    with torch.cuda.device(dev):
+        _native.call("tio_keep_largest", _ptr(data), code, b, vox, mode, _ptr(keys_d), n, key, has_key, _ptr(roots),
+                     _ptr(count), _ptr(winner), fill_ptr, _stream(data))
+    _count(2)
+    del keep
+    return data, roots

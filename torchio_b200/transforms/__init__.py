@@ -5,7 +5,7 @@ from .compose import Compose
 from .histogram import HistogramStandardization, compute_histogram_landmarks
 from .intensity import (BiasField, Blur, Gamma, LabelsToImage, Noise, Normalize, RescaleIntensity, Standardize,
                         ZNormalization)
-from .label import Contour, OneHot, RemapLabels, RemoveLabels, SequentialLabels
+from .label import Contour, KeepLargestComponent, OneHot, RemapLabels, RemoveLabels, SequentialLabels
 from .inverse import apply_inverse_transform, get_inverse_transform
 from .neighbours import Crop, CropOrPad, Flip, Pad
 from .resolution import Anisotropy, Resize
@@ -13,7 +13,7 @@ from .spatial import Affine, ElasticDeformation, Resample, Spatial
 
 __all__ = [
     "Affine", "Anisotropy", "AppliedTransform", "BiasField", "Blur", "Clamp", "Compose", "Contour", "Crop", "CropOrPad", "ElasticDeformation",
-    "Flip", "Gamma", "HistogramStandardization", "IntensityTransform", "LabelsToImage", "Mask", "Noise", "Normalize", "OneHot", "Pad", "RemapLabels",
+    "Flip", "Gamma", "HistogramStandardization", "IntensityTransform", "KeepLargestComponent", "LabelsToImage", "Mask", "Noise", "Normalize", "OneHot", "Pad", "RemapLabels",
     "RemoveLabels", "Resample", "Resize", "RescaleIntensity", "SequentialLabels", "Spatial",
     "SpatialTransform", "Standardize", "Swap", "Transform", "ZNormalization",
     "apply_inverse_transform", "compute_histogram_landmarks", "execution_device", "get_inverse_transform",

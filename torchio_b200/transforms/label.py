@@ -1,11 +1,12 @@
 """Label-map utilities (transforms/label/ of TorchIO 2.0.0a2): RemapLabels, RemoveLabels,
-SequentialLabels, OneHot, Contour and the private inverses.
+SequentialLabels, OneHot, Contour, KeepLargestComponent and the private inverses.
 
 Constructors, ``make_params``, params schema, gating (one batch-wide coin) and history are the
 reference's; only `LabelMap` batches are touched, and, as in the reference, ``include`` /
 ``exclude`` are recorded but not applied.  Each ``apply_transform`` is one pass of a CUDA kernel:
 a table lookup (`ops.label_lut`, tables built by `tables.label_lut` with torch's own scalar
-rules), the 27-point contour stencil, the one-hot expansion or the channel argmax.
+rules), the 27-point contour stencil, the one-hot expansion, the channel argmax, or (KeepLargestComponent)
+a batched connected-component union-find.
 """
 
 from __future__ import annotations
@@ -204,4 +205,36 @@ class Contour(Transform):
     def apply_transform(self, batch: SubjectsBatch, params: dict[str, Any]) -> SubjectsBatch:
         for _, ib in _label_batches(batch):
             ib.data = ops.label_contour(ib.data)
+        return batch
+
+
+class KeepLargestComponent(Transform):
+    """Within each label of each single-channel label map, set every connected component but the
+    largest to ``background_label`` (label/keep_largest.py:17-125).  ``labels=None`` takes every
+    value with ``int(v) != background_label``; ``fully_connected`` selects 26 neighbours, else 6.
+    Among components of equal size the one whose first voxel in C order comes first is kept.
+
+    Every label of every element is labelled in one union-find on the device (`ops.keep_largest`),
+    in place: a transform called with ``copy=True`` (the default) or inside a `Compose` has already
+    copied the batch."""
+
+    def __init__(self, labels: Sequence[int] | None = None, *, background_label: int = 0,
+                 fully_connected: bool = True, **kwargs: Any) -> None:
+        super().__init__(**kwargs)
+        self.labels = list(labels) if labels is not None else None
+        self.background_label = background_label
+        self.fully_connected = fully_connected
+
+    def supports_chunks(self, batch: SubjectsBatch) -> bool:
+        return True  # elements are independent
+
+    def make_params(self, batch: SubjectsBatch) -> dict[str, Any]:
+        return {}
+
+    def apply_transform(self, batch: SubjectsBatch, params: dict[str, Any]) -> SubjectsBatch:
+        for _, ib in _label_batches(batch):
+            channels = ib.data.shape[1]
+            if channels != 1:
+                raise RuntimeError(f"KeepLargestComponent requires single-channel label maps, got {channels} channels")
+            ib.data, _ = ops.keep_largest(ib.data, self.labels, self.background_label, self.fully_connected)
         return batch
