@@ -153,6 +153,18 @@ int tio_remap(const void* src, void* dst, int elem_bytes, int B, int C, int I, i
               const void* fill, const uint8_t* flip, void* stream);
 
 /*
+ * Axis permutation with flips of a (B,C,I,J,K) batch into (B,C,n[perm0],n[perm1],n[perm2]),
+ * n = (I,J,K): out[b,c,o0,o1,o2] = in[b,c,s] with s[perm_d] = o_d, or n[perm_d]-1-o_d when bit
+ * perm_d of `flip_bits` is set (flips are indexed by INPUT axis: flip first, then transpose).
+ * Replaces torch.flip per axis + permute(...).contiguous() (spatial/reorient.py:63-91) and
+ * permute(0,1,4,3,2).contiguous() (transpose.py:36-50) with one pass over the batch.  Any dtype by
+ * size (`elem_bytes` in {1,2,4,8}).  `perm` must be a permutation of (0,1,2) other than the
+ * identity (flips alone are tio_remap's), `flip_bits` in 0..7; src and dst must not overlap.
+ */
+int tio_permute(const void* src, void* dst, int elem_bytes, int B, int C, int I, int J, int K,
+                int perm0, int perm1, int perm2, int flip_bits, void* stream);
+
+/*
  * Parameter-table upload without the copy engine: an SM kernel reads `bytes`
  * from page-locked host memory (`host_pinned`, a cudaHostAlloc/cudaHostRegister
  * pointer, device-visible under unified addressing) and writes them to

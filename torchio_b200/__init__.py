@@ -5,7 +5,8 @@ Drop-in for the reference's spatial + intensity augmentation chain
 `Noise`, `Gamma`, `Compose`), the label-map utilities (`RemapLabels`, `RemoveLabels`,
 `SequentialLabels`, `OneHot`, `Contour`, `KeepLargestComponent`), the resolution changes (`Anisotropy`,
 `Resize`), histogram standardization (`HistogramStandardization`,
-`ZNormalization`), `Clamp`, `Mask`, `Swap` and its patch path (`UniformSampler`, `Queue`,
+`ZNormalization`), `Clamp`, `Mask`, `Swap`, the orientation and shape
+utilities (`Reorient`, `Transpose`, `EnsureShapeMultiple`, `CopyAffine`, `ToReferenceSpace`) and its patch path (`UniformSampler`, `Queue`,
 `SubjectsLoader`) on tensor-backed `Subject` / `SubjectsBatch` data.  The
 tensor math runs in hand-written sm_90a (H100) CUDA kernels exposed through the C-ABI
 of ``include/tio_b200.h``; see DESIGN.md and INTEGRATION.md.
@@ -18,22 +19,22 @@ from .params import Choice
 from .patches import (GridSampler, ImagesLoader, LabelSampler, PatchLocation, PatchSampler, Queue,
                       StudiesLoader, SubjectsLoader, UniformSampler, WeightedSampler, collate_images, collate_studies,
                       collate_subjects)
-from .transforms import (Affine, Anisotropy, AppliedTransform, BiasField, Blur, Clamp, Compose, Contour, Crop, CropOrPad,
-                         ElasticDeformation, Flip, Gamma, HistogramStandardization, IntensityTransform, KeepLargestComponent, LabelsToImage, Mask, Noise, Normalize, OneHot, Pad,
-                         RemapLabels, RemoveLabels, Resample, RescaleIntensity, Resize, SequentialLabels, Spatial,
-                         SpatialTransform, Swap, Standardize, Transform, ZNormalization,
+from .transforms import (Affine, Anisotropy, AppliedTransform, BiasField, Blur, Clamp, Compose, Contour, CopyAffine, Crop, CropOrPad,
+                         ElasticDeformation, EnsureShapeMultiple, Flip, Gamma, HistogramStandardization, IntensityTransform, KeepLargestComponent, LabelsToImage, Mask, Noise, Normalize, OneHot, Pad,
+                         RemapLabels, RemoveLabels, Reorient, Resample, RescaleIntensity, Resize, SequentialLabels, Spatial,
+                         SpatialTransform, Swap, Standardize, ToReferenceSpace, Transform, Transpose, ZNormalization,
                          apply_inverse_transform, execution_device, get_inverse_transform,
                          set_execution_device)
 
 __version__ = "0.1.0"
 
 __all__ = [
-    "Affine", "AffineMatrix", "Anisotropy", "AppliedTransform", "BiasField", "Blur", "Choice", "Clamp", "Compose", "Contour", "Crop", "CropOrPad",
-    "ElasticDeformation", "Flip", "Gamma", "GridSampler", "HistogramStandardization", "Image", "ImagesBatch", "ImagesLoader", "IntensityTransform",
+    "Affine", "AffineMatrix", "Anisotropy", "AppliedTransform", "BiasField", "Blur", "Choice", "Clamp", "Compose", "Contour", "CopyAffine", "Crop", "CropOrPad",
+    "ElasticDeformation", "EnsureShapeMultiple", "Flip", "Gamma", "GridSampler", "HistogramStandardization", "Image", "ImagesBatch", "ImagesLoader", "IntensityTransform",
     "KeepLargestComponent",     "LabelMap", "LabelSampler", "LabelsToImage", "Mask", "Noise", "Normalize", "OneHot", "Pad", "PatchLocation", "PatchSampler", "Queue", "RemapLabels", "RemoveLabels",
-    "Resample", "RescaleIntensity", "Resize", "ScalarImage", "SequentialLabels", "Spatial",
+    "Reorient", "Resample", "RescaleIntensity", "Resize", "ScalarImage", "SequentialLabels", "Spatial",
     "SpatialTransform", "Standardize", "StudiesBatch", "StudiesLoader", "Subject", "SubjectsBatch",
-    "SubjectsLoader", "Swap", "Transform", "UniformSampler", "WeightedSampler", "ZNormalization", "apply_inverse_transform", "collate_images",
+    "SubjectsLoader", "Swap", "ToReferenceSpace", "Transform", "Transpose", "UniformSampler", "WeightedSampler", "ZNormalization", "apply_inverse_transform", "collate_images",
     "collate_studies", "collate_subjects", "exact_coords_default", "execution_device", "get_inverse_transform",
     "set_exact_coords", "set_execution_device",
 ]

@@ -67,6 +67,7 @@ _SIGNATURES = {
     "tio_components": [c_void_p] + [c_int] * 6 + [c_void_p, c_int, c_int64, c_int, c_int] + [c_void_p] * 4,
     "tio_component_roots": [c_void_p, c_int, c_int, c_int64] + [c_void_p] * 4,
     "tio_keep_largest": [c_void_p, c_int, c_int, c_int64, c_int, c_void_p, c_int, c_int64, c_int] + [c_void_p] * 5,
+    "tio_permute": [c_void_p, c_void_p] + [c_int] * 10 + [c_void_p],
 }
 
 _lib = None

@@ -26,6 +26,67 @@ from torch import Tensor
 
 _BATCH_META_KEYS = ("_batch_size", "_batched_keys", "_keep")
 
+# ---- nibabel.orientations, restated (the reference's Reorient and AffineMatrix.orientation) ----
+# An "ornt" is a (3, 2) float64 array: row = input axis, [output axis, +1 / -1 direction].
+_AXIS_LABELS = (("L", "R"), ("P", "A"), ("I", "S"))
+
+
+def _io_orientation(affine: np.ndarray) -> np.ndarray:
+    """Axis permutation and flips closest to the direction part of ``affine``: polar decomposition
+    by SVD, then per input axis the output axis of largest magnitude, taken greedily."""
+    rzs = np.asarray(affine, dtype=np.float64)[:3, :3]
+    zooms = np.sqrt(np.sum(rzs * rzs, axis=0))
+    zooms[zooms == 0] = 1
+    rs = rzs / zooms
+    p, s, qs = np.linalg.svd(rs, full_matrices=False)
+    keep = s > s.max() * 3 * np.finfo(s.dtype).eps
+    r = np.dot(p[:, keep], qs[keep])
+    ornt = np.ones((3, 2), dtype=np.int8) * np.nan
+    for in_ax in range(3):
+        col = r[:, in_ax]
+        if not np.allclose(col, 0):
+            out_ax = np.argmax(np.abs(col))
+            ornt[in_ax, 0] = out_ax
+            ornt[in_ax, 1] = -1 if col[out_ax] < 0 else 1
+            r[out_ax, :] = 0
+    return ornt
+
+
+def _axcodes2ornt(axcodes) -> np.ndarray:
+    """Orientation of axis codes such as "RAS" (L/P/I = −1, R/A/S = +1)."""
+    ornt = np.ones((len(axcodes), 2), dtype=np.int8) * np.nan
+    for code_idx, code in enumerate(axcodes):
+        for label_idx, codes in enumerate(_AXIS_LABELS):
+            if code in codes:
+                ornt[code_idx, :] = [label_idx, -1 if code == codes[0] else 1]
+                break
+    return ornt
+
+
+def _ornt_transform(start_ornt: np.ndarray, end_ornt: np.ndarray) -> np.ndarray:
+    """The orientation that takes data in ``start_ornt`` to ``end_ornt``."""
+    result = np.empty_like(start_ornt)
+    for end_in_idx, (end_out_idx, end_flip) in enumerate(end_ornt):
+        for start_in_idx, (start_out_idx, start_flip) in enumerate(start_ornt):
+            if end_out_idx == start_out_idx:
+                result[start_in_idx, :] = [end_in_idx, 1 if start_flip == end_flip else -1]
+                break
+        else:
+            raise ValueError("Unable to find out axis %d in start_ornt" % end_out_idx)
+    return result
+
+
+def _inv_ornt_aff(ornt: np.ndarray, shape) -> np.ndarray:
+    """Affine from the voxel grid after applying ``ornt`` to an array of ``shape`` back to the
+    original grid: undo the transpose, then the flips about the array's centre."""
+    shape = np.array(shape)[:3]
+    axis_transpose = [int(v) for v in ornt[:, 0]]
+    undo_reorder = np.eye(4)[axis_transpose + [3], :]
+    undo_flip = np.diag(list(ornt[:, 1]) + [1.0])
+    center_trans = -(shape - 1) / 2.0
+    undo_flip[:3, 3] = (ornt[:, 1] * center_trans) - center_trans
+    return np.dot(undo_flip, undo_reorder)
+
 
 class AffineMatrix:
     """4x4 voxel->world matrix (float64, host)."""
@@ -83,21 +144,10 @@ class AffineMatrix:
     def orientation(self) -> tuple[str, str, str]:
         """Anatomical axis codes, e.g. ('R','A','S') (data/affine.py:124-128 = nibabel's
         aff2axcodes: closest axis permutation/flips of the direction part, via its SVD)."""
-        rzs = self._m[:3, :3].astype(np.float64)
-        zooms = np.sqrt((rzs * rzs).sum(axis=0))
-        zooms[zooms == 0] = 1.0
-        rs = rzs / zooms
-        p, s, qs = np.linalg.svd(rs)
-        keep = s > s.max() * 3 * np.finfo(s.dtype).eps
-        r = p[:, keep] @ qs[keep]
-        labels = (("L", "R"), ("P", "A"), ("I", "S"))
         codes: list[str | None] = [None, None, None]
-        for in_ax in range(3):
-            col = r[:, in_ax]
-            if not np.allclose(col, 0):
-                out_ax = int(np.argmax(np.abs(col)))
-                codes[in_ax] = labels[out_ax][0] if col[out_ax] < 0 else labels[out_ax][1]
-                r[out_ax, :] = 0
+        for in_ax, (out_ax, direction) in enumerate(_io_orientation(self._m)):
+            if not np.isnan(out_ax):
+                codes[in_ax] = _AXIS_LABELS[int(out_ax)][0 if direction < 0 else 1]
         return (codes[0], codes[1], codes[2])
 
     def to(self, *args: Any, **kwargs: Any) -> AffineMatrix:

@@ -338,6 +338,35 @@ def remap(src: Tensor, out_shape, offsets, *, mode: str = "constant", fill=0, fl
     return dst
 
 
+def permute(src: Tensor, perm, flip_bits: int = 0) -> Tensor:
+    """Spatial axis permutation with flips of a (B, C, I, J, K) batch in one pass: output axis d is
+    input axis ``perm[d]``, reversed when bit ``perm[d]`` of ``flip_bits`` is set (flips indexed by
+    input axis, applied before the transpose).  The identity permutation flips through `remap`
+    with the same bits for every element, or returns ``src`` itself when nothing flips, as the
+    reference does.  reorient.py:63-91, transpose.py:36-50."""
+    _require_cuda(src, "permute")
+    if src.ndim != 5:
+        raise ValueError(f"permute expects (B, C, I, J, K), got {tuple(src.shape)}")
+    perm = tuple(int(p) for p in perm)
+    if sorted(perm) != [0, 1, 2]:
+        raise ValueError(f"permute: {perm} is not a permutation of (0, 1, 2)")
+    flip_bits = int(flip_bits)
+    if perm == (0, 1, 2):
+        if flip_bits == 0:
+            return src
+        (flags,) = upload(src.device, np.full(src.shape[0], flip_bits, dtype=np.uint8))
+        return remap(src, src.shape[2:], (0, 0, 0), flip=flags)
+    src = src.contiguous()
+    b, c, i, j, k = (int(v) for v in src.shape)
+    n = (i, j, k)
+    dst = torch.empty((b, c, *(n[p] for p in perm)), dtype=src.dtype, device=src.device)
+    with torch.cuda.device(src.device):
+        _native.call("tio_permute", _ptr(src), _ptr(dst), src.element_size(), b, c, i, j, k, *perm, flip_bits,
+                     _stream(src))
+    _count(1)
+    return dst
+
+
 def blur(src: Tensor, taps: Tensor, radius: Tensor, big_r: int, axes_mask: int,
          identity: Tensor | None) -> Tensor:
     """K3 (intensity/blur.py:129-252)."""

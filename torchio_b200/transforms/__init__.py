@@ -8,14 +8,15 @@ from .intensity import (BiasField, Blur, Gamma, LabelsToImage, Noise, Normalize,
 from .label import Contour, KeepLargestComponent, OneHot, RemapLabels, RemoveLabels, SequentialLabels
 from .inverse import apply_inverse_transform, get_inverse_transform
 from .neighbours import Crop, CropOrPad, Flip, Pad
+from .orientation import CopyAffine, EnsureShapeMultiple, Reorient, ToReferenceSpace, Transpose
 from .resolution import Anisotropy, Resize
 from .spatial import Affine, ElasticDeformation, Resample, Spatial
 
 __all__ = [
-    "Affine", "Anisotropy", "AppliedTransform", "BiasField", "Blur", "Clamp", "Compose", "Contour", "Crop", "CropOrPad", "ElasticDeformation",
+    "Affine", "Anisotropy", "AppliedTransform", "BiasField", "Blur", "Clamp", "Compose", "Contour", "CopyAffine", "Crop", "CropOrPad", "ElasticDeformation", "EnsureShapeMultiple",
     "Flip", "Gamma", "HistogramStandardization", "IntensityTransform", "KeepLargestComponent", "LabelsToImage", "Mask", "Noise", "Normalize", "OneHot", "Pad", "RemapLabels",
-    "RemoveLabels", "Resample", "Resize", "RescaleIntensity", "SequentialLabels", "Spatial",
-    "SpatialTransform", "Standardize", "Swap", "Transform", "ZNormalization",
+    "RemoveLabels", "Reorient", "Resample", "Resize", "RescaleIntensity", "SequentialLabels", "Spatial",
+    "SpatialTransform", "Standardize", "Swap", "ToReferenceSpace", "Transform", "Transpose", "ZNormalization",
     "apply_inverse_transform", "compute_histogram_landmarks", "execution_device", "get_inverse_transform",
     "set_execution_device",
 ]
