@@ -505,6 +505,48 @@ int tio_keep_largest(void* data, int dtype, int B, int64_t vox, int mode, const 
                      int n_keys, int64_t background, int has_background, const uint32_t* parent,
                      const uint32_t* count, uint64_t* winner, const void* fill, void* stream);
 
+/*
+ * Spike (intensity/spike.py:124-223 of the reference: fftn of data.float(), fftshift, peak =
+ * |spectrum|.amax() per (b, c), spectrum[idx] += peak * intensity per spike, ifftshift, ifftn, .real,
+ * .to(dtype), torch.where for per-instance gating).  A spike at the fftshift index p of an axis of n
+ * points is frequency f = (p - n / 2) mod n, and its inverse FFT is a plane wave, so
+ *   out[b, c, i, j, k] = x + A[b, c] * sum_s cos(2 pi (u_s i / I + v_s j / J + w_s k / K)),
+ *   A[b, c] = peak[b, c] * intensity[b] / (I J K),
+ * with x = float(data) and peak = sum(x) when no voxel of the row is negative.  `data` / `src` is a
+ * contiguous (B, C, I, J, K) batch of any tio_dtype; B * C <= 65535.  `intensity` is device fp32 [B]:
+ * an element with intensity 0 is not active, and no call reads or writes its voxels.
+ *
+ * tio_spike_stats: per row r = b * C + c, sum[r] (device fp64) = sum of float(x) and flags[r]
+ * (device uint32) = bit 0: some voxel < 0, bit 1: some voxel is NaN or +-Inf; both 0 for an inactive
+ * row.  workspace: device scratch of tio_spike_stats_workspace_bytes(B * C) bytes.  The sum is
+ * added in a fixed order: the same input gives the same bits.
+ *
+ * tio_spectrum_peak: peak[r] (device fp32) = max |fftn(float(x))| of every active row whose flags
+ * are exactly 1 (signed and finite), 0 for the others; the rows are chosen on the device.
+ * Forward half-spectrum FFT (bins 0..K/2 on the last axis hold every magnitude of a real input):
+ * a K pass from the input, an in-place J pass and an I pass that only reduces, over a complex64
+ * workspace of [rows][I][J][K/2 + 1]; rows are processed in chunks of workspace_bytes /
+ * (I * J * (K/2 + 1) * 8), at least one.  Every axis is at most 4096 points.
+ *
+ * tio_spike: in place, each voxel of an active row gets x + A cos(...) cast back as the reference's
+ * .to(dtype); a row with flags bit 1 becomes all NaN (the reference's FFT spreads the value).
+ *   spikes  device int32 [B][S][4]: u, v, w (frequencies, 0 <= f < axis length), 1; an element's
+ *           list is followed by (0, 0, 0, 0) padding up to the longest list
+ *   sum, flags, peak  from tio_spike_stats / tio_spectrum_peak; A uses peak when flags bit 0 is set
+ *   tables  device scratch of B * S * (I + J + K) * 8 bytes: the per-axis phase tables
+ *           exp(2 pi i (f n mod L) / L), kept in shared memory when one element's fit in 96 KiB
+ */
+size_t tio_spike_stats_workspace_bytes(int rows);
+int tio_spike_stats(const void* src, int dtype, int B, int C, int64_t vox, const float* intensity,
+                    double* sum, uint32_t* flags, void* workspace, size_t workspace_bytes,
+                    void* stream);
+int tio_spectrum_peak(const void* src, int dtype, int B, int C, int I, int J, int K,
+                      const float* intensity, const uint32_t* flags, float* peak, void* workspace,
+                      size_t workspace_bytes, void* stream);
+int tio_spike(void* data, int dtype, int B, int C, int I, int J, int K, const int32_t* spikes, int S,
+              const float* intensity, const double* sum, const uint32_t* flags, const float* peak,
+              void* tables, size_t tables_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

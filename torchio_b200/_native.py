@@ -68,6 +68,10 @@ _SIGNATURES = {
     "tio_component_roots": [c_void_p, c_int, c_int, c_int64] + [c_void_p] * 4,
     "tio_keep_largest": [c_void_p, c_int, c_int, c_int64, c_int, c_void_p, c_int, c_int64, c_int] + [c_void_p] * 5,
     "tio_permute": [c_void_p, c_void_p] + [c_int] * 10 + [c_void_p],
+    "tio_spike_stats_workspace_bytes": [c_int],
+    "tio_spike_stats": [c_void_p, c_int, c_int, c_int, c_int64] + [c_void_p] * 4 + [c_size_t, c_void_p],
+    "tio_spectrum_peak": [c_void_p] + [c_int] * 6 + [c_void_p] * 4 + [c_size_t, c_void_p],
+    "tio_spike": [c_void_p] + [c_int] * 6 + [c_void_p, c_int] + [c_void_p] * 5 + [c_size_t, c_void_p],
 }
 
 _lib = None

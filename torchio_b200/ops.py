@@ -1013,3 +1013,77 @@ def keep_largest(data: Tensor, labels, background_label, fully_connected: bool) 
     _count(2)
     del keep
     return data, roots
+
+
+# ---- Spike (intensity/spike.py) -----------------------------------------------------------------
+
+SPIKE_MAX_AXIS = 4096              # tio_spectrum_peak's longest axis
+SPECTRUM_WORKSPACE_BYTES = 512 << 20  # half-spectrum rows are transformed in chunks of about this size
+
+
+def spike(data: Tensor, spikes: np.ndarray, intensity: np.ndarray) -> Tensor:
+    """In place on a contiguous (B, C, I, J, K) CUDA batch of any image dtype: the reference's
+    `_add_spikes` (spike.py:124-223) as x + A cos(...) per spike, with A = peak * intensity / (I J K)
+    and peak = max |fftn(x.float())| of each (b, c), the sum when no voxel is negative.  ``spikes``:
+    int32 (B, S, 4) rows ``u, v, w, 1`` (frequencies) padded with zeros, ``intensity``: fp32 (B,),
+    0 for an element that stays untouched.  Stats, spectrum peak and spike pass stay on the device:
+    no host sync."""
+    _require_cuda(data, "spike")
+    if data.dtype not in RESOLUTION_DTYPE_CODES:
+        raise TypeError(f"spike: unsupported dtype {data.dtype}")
+    if data.ndim != 5 or not data.is_contiguous():
+        raise ValueError(f"spike expects a contiguous (B, C, I, J, K) batch, got {tuple(data.shape)}")
+    b, c, i, j, k = (int(s) for s in data.shape)
+    if max(i, j, k) > SPIKE_MAX_AXIS:
+        raise NotImplementedError(
+            f"Spike: spatial shape {(i, j, k)} has an axis longer than {SPIKE_MAX_AXIS} points, the"
+            f" longest the spectrum peak supports")
+    spikes = np.ascontiguousarray(spikes, dtype=np.int32)
+    intensity = np.ascontiguousarray(intensity, dtype=np.float32)
+    if spikes.ndim != 3 or spikes.shape[0] != b or spikes.shape[2] != 4 or intensity.shape != (b,):
+        raise ValueError(f"spike: tables {spikes.shape} / {intensity.shape} for a batch of {b}")
+    if data.numel() == 0 or spikes.shape[1] == 0:
+        return data
+    s = int(spikes.shape[1])
+    spikes_d, intensity_d = upload(data.device, spikes, intensity)
+    total, flags = spike_stats(data, intensity_d)
+    peak = spectrum_peak(data, intensity_d, flags)
+    tables_bytes = b * s * (i + j + k) * 8
+    tables = torch.empty(tables_bytes, dtype=torch.uint8, device=data.device)
+    with torch.cuda.device(data.device):
+        _native.call("tio_spike", _ptr(data), RESOLUTION_DTYPE_CODES[data.dtype], b, c, i, j, k, _ptr(spikes_d), s,
+                     _ptr(intensity_d), _ptr(total), _ptr(flags), _ptr(peak), _ptr(tables), tables_bytes,
+                     _stream(data))
+    _count(2)
+    return data
+
+
+def spike_stats(data: Tensor, intensity: Tensor) -> tuple[Tensor, Tensor]:
+    """(sum fp64 (B*C,), flags int32 (B*C,)) of `tio_spike_stats` for a contiguous (B, C, ...) CUDA
+    batch; ``intensity``: fp32 (B,) on the device, 0 for an inactive element."""
+    b, c = int(data.shape[0]), int(data.shape[1])
+    total = torch.empty(b * c, dtype=torch.float64, device=data.device)
+    flags = torch.empty(b * c, dtype=torch.int32, device=data.device)
+    ws_bytes = _native.lib().tio_spike_stats_workspace_bytes(b * c)
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=data.device)
+    with torch.cuda.device(data.device):
+        _native.call("tio_spike_stats", _ptr(data), RESOLUTION_DTYPE_CODES[data.dtype], b, c, data[0, 0].numel(),
+                     _ptr(intensity), _ptr(total), _ptr(flags), _ptr(ws), ws_bytes, _stream(data))
+    _count(2)
+    return total, flags
+
+
+def spectrum_peak(data: Tensor, intensity: Tensor, flags: Tensor, workspace_bytes: int | None = None) -> Tensor:
+    """peak fp32 (B*C,) of `tio_spectrum_peak`: max |fftn(x.float())| of the active rows whose flags
+    are 1 (signed and finite), 0 elsewhere; ``workspace_bytes`` bounds the half-spectrum chunk."""
+    b, c, i, j, k = (int(s) for s in data.shape)
+    row_bytes = i * j * (k // 2 + 1) * 8
+    if workspace_bytes is None:
+        workspace_bytes = min(b * c, max(1, SPECTRUM_WORKSPACE_BYTES // row_bytes)) * row_bytes
+    peak = torch.empty(b * c, dtype=torch.float32, device=data.device)
+    ws = torch.empty(workspace_bytes, dtype=torch.uint8, device=data.device)
+    with torch.cuda.device(data.device):
+        _native.call("tio_spectrum_peak", _ptr(data), RESOLUTION_DTYPE_CODES[data.dtype], b, c, i, j, k,
+                     _ptr(intensity), _ptr(flags), _ptr(peak), _ptr(ws), workspace_bytes, _stream(data))
+    _count(1 + 3 * -(-(b * c) // (workspace_bytes // row_bytes)))
+    return peak
