@@ -547,6 +547,25 @@ int tio_spike(void* data, int dtype, int B, int C, int I, int J, int K, const in
               const float* intensity, const double* sum, const uint32_t* flags, const float* peak,
               void* tables, size_t tables_bytes, void* stream);
 
+/*
+ * Ghosting (intensity/ghosting.py:149-277 of the reference: fftn of data.float(), fftshift, times a
+ * real mask that varies along one axis, ifftshift, ifftn, .real, .to(dtype), torch.where for
+ * per-instance gating).  The FFTs over the other two axes cancel, so each line along the ghosted
+ * axis (n points) becomes
+ *   out = Re(ifft_n(H fft_n(x))) = ifft_n(Hs fft_n(x)),   Hs(f) = (H(f) + H(-f mod n)) / 2,
+ * with x = float(data) and H = ifftshift(line_mask) (ghosting.py:190-197, 251-271).  In place on a
+ * contiguous (B, C, I, J, K) batch of any tio_dtype; B * C <= 65535.
+ *   table   device fp32 [B][n_max]: element b's H in unshifted order in its first n entries
+ *   axis    device int32 [B]: element b's ghosted axis (0 = I, 1 = J, 2 = K)
+ *   active  device uint8 [B]: 0 = not active, no voxel of the element is read or written
+ *   axes    bit a set for each axis some active element ghosts (1..7): one launch per set bit;
+ *           each of these axes is at most 4096 points and at most n_max
+ *   flags   device scratch of B * C uint32
+ * A row with a NaN or +-Inf voxel becomes all NaN (the reference's FFT spreads the value).
+ */
+int tio_ghosting(void* data, int dtype, int B, int C, int I, int J, int K, const float* table, int n_max,
+                 const int32_t* axis, const uint8_t* active, int axes, uint32_t* flags, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

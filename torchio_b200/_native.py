@@ -72,6 +72,7 @@ _SIGNATURES = {
     "tio_spike_stats": [c_void_p, c_int, c_int, c_int, c_int64] + [c_void_p] * 4 + [c_size_t, c_void_p],
     "tio_spectrum_peak": [c_void_p] + [c_int] * 6 + [c_void_p] * 4 + [c_size_t, c_void_p],
     "tio_spike": [c_void_p] + [c_int] * 6 + [c_void_p, c_int] + [c_void_p] * 5 + [c_size_t, c_void_p],
+    "tio_ghosting": [c_void_p] + [c_int] * 6 + [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p],
 }
 
 _lib = None

@@ -1087,3 +1087,47 @@ def spectrum_peak(data: Tensor, intensity: Tensor, flags: Tensor, workspace_byte
                      _ptr(intensity), _ptr(flags), _ptr(peak), _ptr(ws), workspace_bytes, _stream(data))
     _count(1 + 3 * -(-(b * c) // (workspace_bytes // row_bytes)))
     return peak
+
+
+# ---- Ghosting (intensity/ghosting.py) -----------------------------------------------------------
+
+GHOSTING_MAX_AXIS = 4096  # longest line tio_ghosting's shared-memory FFT holds
+
+
+def ghosting(data: Tensor, table: np.ndarray, axis: np.ndarray, active: np.ndarray) -> Tensor:
+    """In place on a contiguous (B, C, I, J, K) CUDA batch of any image dtype: the reference's
+    `_add_ghosting` / `_add_ghosting_per_element` (ghosting.py:149-277) as one filter per line
+    along each element's axis, ``ifft(Hs * fft(x))``.  ``table``: fp32 (B, n_max), element b's
+    ``ifftshift(line_mask)`` in its first ``shape[axis[b]]`` entries; ``axis``: (B,) in 0..2;
+    ``active``: (B,) bool, False for an element that stays untouched.  No host sync."""
+    _require_cuda(data, "ghosting")
+    if data.dtype not in RESOLUTION_DTYPE_CODES:
+        raise TypeError(f"ghosting: unsupported dtype {data.dtype}")
+    if data.ndim != 5 or not data.is_contiguous():
+        raise ValueError(f"ghosting expects a contiguous (B, C, I, J, K) batch, got {tuple(data.shape)}")
+    b, c, i, j, k = (int(s) for s in data.shape)
+    table = np.ascontiguousarray(table, dtype=np.float32)
+    axis = np.ascontiguousarray(axis, dtype=np.int32)
+    active = np.ascontiguousarray(active, dtype=np.uint8)
+    if table.ndim != 2 or table.shape[0] != b or axis.shape != (b,) or active.shape != (b,):
+        raise ValueError(f"ghosting: tables {table.shape} / {axis.shape} / {active.shape} for a batch of {b}")
+    ghosted = sorted({int(a) for a, on in zip(axis, active, strict=True) if on})
+    if not ghosted or data.numel() == 0:
+        return data
+    if ghosted[0] < 0 or ghosted[-1] > 2:
+        raise ValueError(f"ghosting: axis {ghosted[0] if ghosted[0] < 0 else ghosted[-1]} outside 0..2")
+    longest = max(data.shape[2 + a] for a in ghosted)
+    if longest > GHOSTING_MAX_AXIS:
+        raise NotImplementedError(
+            f"Ghosting: spatial shape {(i, j, k)} is ghosted along an axis longer than {GHOSTING_MAX_AXIS} points,"
+            f" the longest the line FFT supports")
+    if table.shape[1] < longest:
+        raise ValueError(f"ghosting: table rows of {table.shape[1]} entries for an axis of {longest} points")
+    table_d, axis_d, active_d = upload(data.device, table, axis, active)
+    flags = torch.empty(b * c, dtype=torch.int32, device=data.device)
+    with torch.cuda.device(data.device):
+        _native.call("tio_ghosting", _ptr(data), RESOLUTION_DTYPE_CODES[data.dtype], b, c, i, j, k, _ptr(table_d),
+                     int(table.shape[1]), _ptr(axis_d), _ptr(active_d), sum(1 << a for a in ghosted), _ptr(flags),
+                     _stream(data))
+    _count(2 + len(ghosted))
+    return data
