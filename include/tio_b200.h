@@ -314,7 +314,8 @@ int tio_histogram_map(const void* src, void* dst, int dtype, int B, int64_t per_
  *       (transforms/intensity/gamma.py:88-90)
  *   per-element identity rows (bias_identity[b], all radii 0, keep[b] == 0,
  *   gamma[b] == 1) pass through every stage as bit-exact copies
- *   scratch: B*C*I*J*K floats, required when axes_mask has bit 1 or 2 (J/K), or
+ *   scratch: B*C*I*J*K floats, required when axes_mask has bit 1 or 2 (J/K) together with
+ *            bias or bit 0 (J/K alone reads src directly), or
  *            when R > 16 with blur and bias both active, or more than one axis
  * src, dst, scratch must be distinct when blur is active.
  */
@@ -327,6 +328,30 @@ int tio_intensity_fused(const float* src, float* dst, float* scratch,
                         const float* z, const float* z2,
                         uint64_t philox_seed, int noise_mode, int rician,
                         const float* gamma, void* stream);
+
+/*
+ * The first pass of the chain above (K2 bias and the I axis of K3: dst = what tio_intensity_fused
+ * hands to its J/K pass) and z = stream elements [offset, offset+n) of tio_randn_mt19937(seed),
+ * from one persistent kernel in which the two share every SM: the pass is bound by HBM, the
+ * normals by instruction issue, so together they take little more than the slower one alone.
+ * Both outputs are bit-identical to what tio_intensity_fused (axes_mask & 1, no noise, no gamma)
+ * and tio_randn_mt19937 write.  The chain is finished by tio_intensity_fused(dst -> out) with
+ * axes_mask & 6, no bias, and z as the supplied normals.
+ *   taps / radius / R / axes_mask as for tio_blur; only bit 0 (the I axis) is read; R <= 6
+ *   K % 4 == 0; src, dst, z 16-byte aligned; src != dst
+ *   seed / offset / n / table as for tio_randn_mt19937; z holds n floats
+ *   workspace  device scratch of tio_intensity_pass1_with_normals_workspace_bytes(offset, n)
+ * Anything else (wider tables, ragged rows) is refused; callers then use the two calls above.
+ */
+size_t tio_intensity_pass1_with_normals_workspace_bytes(uint64_t offset, uint64_t n);
+int tio_intensity_pass1_with_normals(const float* src, float* dst,
+                                     int B, int C, int I, int J, int K,
+                                     const float* coarse, int si, int sj, int sk,
+                                     const uint8_t* bias_identity, int bias_divide,
+                                     const float* taps, const int32_t* radius, int R, int axes_mask,
+                                     uint64_t seed, uint64_t offset, uint64_t n, float* z,
+                                     const void* table, void* workspace, size_t workspace_bytes,
+                                     void* stream);
 
 /*
  * LabelsToImage in one pass: dst (B, 1, vox) fp32 from channel 0 of `labels` (B, C, vox) of

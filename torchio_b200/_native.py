@@ -49,6 +49,11 @@ _SIGNATURES = {
     + [c_void_p, c_int, c_int, c_int, c_void_p, c_int]
     + [c_void_p, c_void_p, c_int, c_int]
     + [c_void_p] * 5 + [c_uint64, c_int, c_int, c_void_p, c_void_p],
+    "tio_intensity_pass1_with_normals_workspace_bytes": [c_uint64, c_uint64],
+    "tio_intensity_pass1_with_normals": [c_void_p, c_void_p] + [c_int] * 5
+    + [c_void_p, c_int, c_int, c_int, c_void_p, c_int]
+    + [c_void_p, c_void_p, c_int, c_int]
+    + [c_uint64, c_uint64, c_uint64, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p],
     "tio_labels_to_image": [c_void_p, c_int, c_int, c_int, c_int64, c_void_p, c_int, c_void_p, c_void_p, c_void_p,
                             c_uint64, c_int, c_void_p, c_void_p],
     "tio_label_lut": [c_void_p, c_void_p, c_int, c_int64, c_void_p, c_void_p, c_int, c_int, c_void_p],

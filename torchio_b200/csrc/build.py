@@ -22,7 +22,7 @@ SOURCES = ["error.cu", "resample.cu", "resample_tile.cu", "resample_fast.cu", "u
            "label_maps.cu", "interpolate.cu", "clamp_mask_swap.cu", "components.cu", "permute.cu", "spike.cu",
            "ghosting.cu"]
 HEADERS = [HERE / "common.cuh", HERE / "resample_common.cuh", HERE / "resample_tile.cuh", HERE / "tma.cuh",
-           HERE / "mt19937_layout.h", HERE / "label_lookup.cuh", HERE / "image_dtype.cuh",
+           HERE / "mt19937_layout.h", HERE / "mt19937_normal.cuh", HERE / "label_lookup.cuh", HERE / "image_dtype.cuh",
            HERE / "fft_lines.cuh",
            ROOT / "include" / "tio_b200.h",
            Path(__file__).resolve()]  # the flags below: objects built for another architecture are rebuilt

@@ -17,6 +17,8 @@
 // Separable passes commute up to fp32 summation order (the reference runs
 // I, J, K; this runs I, K, J): differences are ~1e-7 relative.
 #include "common.cuh"
+#include "mt19937_layout.h"
+#include "mt19937_normal.cuh"
 #include "tma.cuh"
 
 namespace tio {
@@ -721,17 +723,17 @@ march_kernel(const float* __restrict__ src, float* __restrict__ dst, int B, int 
 // -------------------------------------------------------------------------
 constexpr int M6_PF = 8;  // cp.async FIFO depth of march6_kernel (power of two)
 
-template <bool HAS_BIAS, bool EPI>
-__global__ void __launch_bounds__(256, EPI ? 1 : 2)
-march6_kernel(const float* __restrict__ src, float* __restrict__ dst, int B, int C, int I, int J,
-              int K, BlurArgs bl, BiasArgs bi, NoiseArgs nz, const float* __restrict__ gamma) {
-  extern __shared__ __align__(16) float smem[];
+// One tile of pass 1: 256 threads, thread `tid` <-> (row j, columns k..k+3) of volume bc, all I
+// planes.  BAR = 0: the 256 threads are a whole CTA (__syncthreads); BAR > 0: they are part of
+// a larger CTA and meet at named barrier BAR.  `smem`: 16 floats of taps, the coarse bias grid,
+// then the FIFO.
+template <bool HAS_BIAS, bool EPI, int BAR>
+__device__ __forceinline__ void march6_tile(float* smem, const int tid, const int k, const int j, const int bc,
+                                            const float* __restrict__ src, float* __restrict__ dst, int B,
+                                            int C, int I, int J, int K, const BlurArgs& bl, const BiasArgs& bi,
+                                            const NoiseArgs& nz, const float* __restrict__ gamma) {
   constexpr int W = 2 * F_R + 1;
-  const int bc = blockIdx.z;
   const int b = bc / C;
-  const int tid = threadIdx.y * blockDim.x + threadIdx.x;
-  const int k = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
-  const int j = blockIdx.y * blockDim.y + threadIdx.y;
   const int64_t n = (int64_t)I * J * K;
   const float* x = src + (int64_t)bc * n;
   float* y = dst + (int64_t)bc * n;
@@ -749,7 +751,8 @@ march6_kernel(const float* __restrict__ src, float* __restrict__ dst, int B, int
     const float* gs = bi.coarse + (int64_t)bc * ns;
     for (int t = tid; t < ns; t += 256) g[t] = gs[t];
   }
-  __syncthreads();
+  if (BAR == 0) __syncthreads();
+  else asm volatile("bar.sync %0, 256;" ::"n"(BAR) : "memory");
   if (k >= K || j >= J) return;
 
   const bool noise_on = EPI && nz.mode != 0 && (!nz.keep || nz.keep[b]);
@@ -905,6 +908,76 @@ march6_kernel(const float* __restrict__ src, float* __restrict__ dst, int B, int
         }
         finish(o, acc);
       }
+    }
+  }
+}
+
+template <bool HAS_BIAS, bool EPI>
+__global__ void __launch_bounds__(256, EPI ? 1 : 2)
+march6_kernel(const float* __restrict__ src, float* __restrict__ dst, int B, int C, int I, int J,
+              int K, BlurArgs bl, BiasArgs bi, NoiseArgs nz, const float* __restrict__ gamma) {
+  extern __shared__ __align__(16) float smem[];
+  march6_tile<HAS_BIAS, EPI, 0>(smem, threadIdx.y * blockDim.x + threadIdx.x,
+                                (blockIdx.x * blockDim.x + threadIdx.x) * 4,
+                                blockIdx.y * blockDim.y + threadIdx.y, blockIdx.z, src, dst, B, C, I, J, K,
+                                bl, bi, nz, gamma);
+}
+
+// -------------------------------------------------------------------------
+// pass 1 and the normal stage of the exact-noise replay (mt19937_normal.cuh) in one persistent
+// kernel, one CTA of 7 warpgroups per SM.  Pass 1 is bound by HBM and leaves most issue slots
+// empty; the normal stage is bound by issue and writes 4 B/voxel.  As two kernels they cannot
+// share an SM (either one's CTAs fill the register file), so here the two roles split one CTA's
+// registers with setmaxnreg: the kernel starts at 72 registers per thread (896 x 72 = 64 512),
+//   warpgroups 0-1  the 256 threads of march6_kernel<HAS_BIAS, false>, raised to 152 registers
+//                   (at 128 the bias variant spills):
+//                   tiles (k-block, j-block, b*c) of that kernel's grid, x fastest, handed out by
+//                   a global counter;
+//   warpgroups 2-6  lowered to 40 registers: the first MT_THREADS threads run segment after
+//                   segment of the normal stage (q = q_lo + blockIdx.x, + gridDim.x, ...), the
+//                   other 64 leave;
+// 256 x 152 + 640 x 40 = 64 512 registers after the exchange.  Both bodies are the device
+// functions the stand-alone kernels run, so the outputs are theirs bit for bit.  Named barriers:
+// 1..5 inside the normal stage, P1N_BAR_SEGMENT between its segments, P1N_BAR_MARCH for pass 1;
+// barrier 0 is never used after the roles part.
+// -------------------------------------------------------------------------
+constexpr int P1N_MARCH_THREADS = 256;
+constexpr int P1N_THREADS = P1N_MARCH_THREADS + 5 * 128;  // 896
+constexpr int P1N_BAR_SEGMENT = 6, P1N_BAR_MARCH = 7;
+constexpr int P1N_RING_FLOATS = MT_RING * MT_N + 4;  // the normal stage's ring, then the tile slot
+
+template <bool HAS_BIAS>
+__global__ void __launch_bounds__(P1N_THREADS, 1)
+pass1_normals_kernel(const float* __restrict__ src, float* __restrict__ dst, int B, int C, int I, int J,
+                     int K, BlurArgs bl, BiasArgs bi, unsigned int* __restrict__ tile_counter,
+                     const uint32_t* __restrict__ states, int q_lo, int q_hi, unsigned long long L,
+                     unsigned long long offset, unsigned long long n, float* __restrict__ z) {
+  extern __shared__ __align__(16) float smem[];
+  if (threadIdx.x < P1N_MARCH_THREADS) {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 152;");
+    const int tid = threadIdx.x;
+    volatile int* next_tile = reinterpret_cast<int*>(smem + MT_RING * MT_N);
+    const int kb_n = (K + 255) / 256, jb_n = (J + 3) / 4;
+    const int tiles = kb_n * jb_n * B * C;
+    for (;;) {
+      if (tid == 0) *next_tile = (int)atomicAdd(tile_counter, 1u);
+      // every thread has left the previous tile: its taps and bias grid may be replaced
+      asm volatile("bar.sync %0, 256;" ::"n"(P1N_BAR_MARCH) : "memory");
+      const int tile = *next_tile;  // rewritten only after the barrier inside march6_tile
+      if (tile >= tiles) break;
+      const int kb = tile % kb_n, jb = (tile / kb_n) % jb_n, bc = tile / (kb_n * jb_n);
+      march6_tile<HAS_BIAS, false, P1N_BAR_MARCH>(smem + P1N_RING_FLOATS, tid, (kb * 64 + (tid & 63)) * 4,
+                                                  jb * 4 + (tid >> 6), bc, src, dst, B, C, I, J, K, bl, bi,
+                                                  NoiseArgs{}, nullptr);
+    }
+  } else {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    const int tid = threadIdx.x - P1N_MARCH_THREADS;
+    if (tid >= MT_THREADS) return;
+    for (int q = q_lo + blockIdx.x; q < q_hi; q += gridDim.x) {
+      mt_normal_segment(reinterpret_cast<uint32_t*>(smem), tid, states, q, L, offset, n, z);
+      // the last consumers have left the ring before the next segment's start state enters it
+      mt_bar_sync<P1N_BAR_SEGMENT, MT_THREADS>();
     }
   }
 }
@@ -1093,11 +1166,13 @@ static int fused_impl(const float* src, float* dst, float* scratch, int B, int C
   if (axes_mask != 0 && bl.R > 16)
     return wide_impl(src, dst, scratch, B, C, I, J, K, bi, bl, axes_mask, nz, gamma, st, who);
   const bool need_jk = (axes_mask & 6) != 0;
-  TIO_CHECK_ARG(!need_jk || (scratch && src != dst && scratch != src && scratch != dst),
-                "%s: blur along J/K needs a scratch buffer and src != dst", who);
-  TIO_CHECK_ARG(!((axes_mask & 1) && src == dst && !need_jk), "%s: blur along I needs src != dst", who);
   const bool need_i = (axes_mask & 1) != 0;
   const bool need_march = !need_jk || need_i || bi.coarse != nullptr;
+  TIO_CHECK_ARG(!need_jk || src != dst, "%s: blur along J/K needs src != dst", who);
+  // J/K alone (the caller ran pass 1 itself: tio_intensity_pass1_with_normals) reads src directly
+  TIO_CHECK_ARG(!(need_jk && need_march) || (scratch && scratch != src && scratch != dst),
+                "%s: blur along J/K after bias or blur along I needs a scratch buffer", who);
+  TIO_CHECK_ARG(!((axes_mask & 1) && src == dst && !need_jk), "%s: blur along I needs src != dst", who);
   const float* cur = src;
   if (need_jk) {
     // checked before any launch
@@ -1189,4 +1264,60 @@ extern "C" int tio_intensity_fused(const float* src, float* dst, float* scratch,
   }
   return fused_impl(src, dst, scratch, B, C, I, J, K, bi, bl, taps ? (axes_mask & 7) : 0, nz,
                     gamma, (cudaStream_t)stream, "tio_intensity_fused");
+}
+
+extern "C" size_t tio_intensity_pass1_with_normals_workspace_bytes(uint64_t offset, uint64_t n) {
+  return tio_randn_mt19937_workspace_bytes(offset, n) + 16;  // start states, then the tile counter
+}
+
+extern "C" int tio_intensity_pass1_with_normals(const float* src, float* dst, int B, int C, int I, int J,
+                                                int K, const float* coarse, int si, int sj, int sk,
+                                                const uint8_t* bias_identity, int bias_divide,
+                                                const float* taps, const int32_t* radius, int R,
+                                                int axes_mask, uint64_t seed, uint64_t offset, uint64_t n,
+                                                float* z, const void* table, void* workspace,
+                                                size_t workspace_bytes, void* stream) {
+  const char* who = "tio_intensity_pass1_with_normals";
+  TIO_CHECK_ARG(src && dst && z, "%s: null src/dst/z", who);
+  TIO_CHECK_ARG(src != dst, "%s: src and dst must not alias", who);
+  TIO_CHECK_ARG(B > 0 && C > 0 && I > 0 && J > 0 && K > 0, "%s: bad shape", who);
+  const bool need_i = taps && (axes_mask & 1);
+  TIO_CHECK_ARG(!need_i || (radius && R >= 0 && R <= F_R), "%s: needs a radius table and R <= %d, got R=%d", who,
+                F_R, R);
+  TIO_CHECK_ARG(K % 4 == 0 && aligned16f(src) && aligned16f(dst) && aligned16f(z),
+                "%s: needs K %% 4 == 0 and 16-byte aligned src, dst and z", who);
+  const int64_t tiles = (int64_t)((K + 255) / 256) * ((J + 3) / 4) * B * C;
+  TIO_CHECK_ARG(tiles < (1ll << 31) - (1 << 20), "%s: batch too large", who);
+  BiasArgs bi{};
+  bi.coarse = coarse; bi.identity = bias_identity; bi.si = si; bi.sj = sj; bi.sk = sk;
+  bi.divide = bias_divide;
+  if (coarse) {
+    bi.sc_i = up_scale(si, I); bi.sc_j = up_scale(sj, J); bi.sc_k = up_scale(sk, K);
+    TIO_CHECK_ARG(si > 0 && sj > 0 && sk > 0 && (size_t)si * sj * sk * 4 <= 64 * 1024,
+                  "%s: coarse bias grid empty or too large", who);
+  }
+  BlurArgs bl{need_i ? taps : nullptr, radius, R};
+  TIO_CHECK_ARG(workspace_bytes >= tio_intensity_pass1_with_normals_workspace_bytes(offset, n),
+                "%s: workspace too small", who);
+  cudaStream_t st = (cudaStream_t)stream;
+  int q_lo, q_hi;
+  const size_t states_bytes = tio_randn_mt19937_workspace_bytes(offset, n);
+  if (int rc = mt_start_states(seed, offset, n, table, workspace, states_bytes, st, who, &q_lo, &q_hi)) return rc;
+  unsigned int* tile_counter = reinterpret_cast<unsigned int*>((char*)workspace + states_bytes);
+  cudaMemsetAsync(tile_counter, 0, sizeof(unsigned int), st);
+  const int ns = coarse ? si * sj * sk : 0;
+  const size_t smem = (size_t)(P1N_RING_FLOATS + 16 + (ns + 3) / 4 * 4) * sizeof(float) + (size_t)M6_PF * 256 * 16;
+  const unsigned long long seg = 1ull << tio_mt::kLog2L;
+  const int grid = num_sms();
+#define TIO_LAUNCH_P1N(BB)                                                                                   \
+  do {                                                                                                       \
+    cudaFuncSetAttribute(pass1_normals_kernel<BB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);  \
+    pass1_normals_kernel<BB><<<grid, P1N_THREADS, smem, st>>>(src, dst, B, C, I, J, K, bl, bi, tile_counter, \
+                                                              (const uint32_t*)workspace, q_lo, q_hi, seg,   \
+                                                              offset, n, z);                                 \
+  } while (0)
+  if (coarse) TIO_LAUNCH_P1N(true); else TIO_LAUNCH_P1N(false);
+#undef TIO_LAUNCH_P1N
+  TIO_CHECK_LAUNCH();
+  return 0;
 }

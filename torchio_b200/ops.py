@@ -528,19 +528,37 @@ def intensity_fused(
     big_r: int = 0, axes_mask: int = 0, mean: Tensor | None = None, std: Tensor | None = None,
     keep: Tensor | None = None, z: Tensor | None = None, z2: Tensor | None = None,
     philox_seed: int = 0, noise_mode: int = 0, rician: bool = False,
-    gamma: Tensor | None = None,
+    gamma: Tensor | None = None, z_replay: tuple[int, int] | None = None,
 ) -> Tensor:
     """Fused bias -> blur -> noise -> gamma (two HBM passes); any stage optional.
 
     Compose-level fusion of consecutive intensity transforms; a single transform
     is a call with only its own stage set.
+
+    ``z_replay`` = (seed, offset) instead of ``z``: the normals are elements
+    [offset, offset + src.numel()) of `randn_mt19937(seed)`.  When the chain has a first pass
+    and a J/K pass of table radius <= 6 on 16-byte aligned rows, the normals are generated
+    inside the first pass (`tio_intensity_pass1_with_normals`) instead of before it; the
+    result is the same bit for bit.
     """
     _require_cuda(src, "intensity_fused")
     src = src.contiguous()
     b, c, i, j, k = src.shape
+    if z_replay is not None:
+        seed, offset = z_replay
+        blur_jk = taps is not None and bool(axes_mask & 6) and big_r <= 6
+        first_pass = coarse is not None or (taps is not None and bool(axes_mask & 1))
+        if (blur_jk and first_pass and noise_mode == 1 and not rician and k % 4 == 0
+                and src.data_ptr() % 16 == 0 and src.numel() % 16 == 0):
+            return _intensity_fused_pass1_normals(
+                src, coarse, bias_identity, bias_divide, taps, radius, big_r, axes_mask, mean, std,
+                keep, gamma, seed, offset)
+        z = randn_mt19937(seed, offset, src.numel(), src.device).view(src.shape)
     dst = torch.empty_like(src)
-    jk = taps is not None and ((axes_mask & 6) or (axes_mask & 7 and big_r > WIDE_R))
-    scratch = torch.empty_like(src) if jk else None
+    # the J/K pass alone reads src directly; after a first pass it reads the scratch buffer
+    two_pass = taps is not None and axes_mask & 6 and (coarse is not None or axes_mask & 1)
+    wide = taps is not None and axes_mask & 7 and big_r > WIDE_R
+    scratch = torch.empty_like(src) if two_pass or wide else None
     si = sj = sk = 0
     if coarse is not None:
         si, sj, sk = coarse.shape[2:]
@@ -555,6 +573,53 @@ def intensity_fused(
         )
     _count(_fused_launches(axes_mask if taps is not None else 0, coarse is not None, big_r))
     return dst
+
+
+def intensity_pass1_with_normals(
+    src: Tensor, seed: int, offset: int, *, coarse: Tensor | None = None,
+    bias_identity: Tensor | None = None, bias_divide: bool = False, taps: Tensor | None = None,
+    radius: Tensor | None = None, big_r: int = 0, axes_mask: int = 0,
+) -> tuple[Tensor, Tensor]:
+    """(first pass of `intensity_fused` on ``src``: bias and the I axis of the blur,
+    elements [offset, offset + src.numel()) of `randn_mt19937(seed)` shaped like ``src``), from one
+    kernel in which the two run side by side on every SM.  Needs table radius <= 6, K % 4 == 0 and
+    16-byte aligned data; the library refuses anything else."""
+    _require_cuda(src, "intensity_pass1_with_normals")
+    src = src.contiguous()
+    b, c, i, j, k = src.shape
+    n = src.numel()
+    if n < 16 or n % 16 or offset % 16 or offset + n > MT_MAX_WORDS:
+        raise ValueError("intensity_pass1_with_normals: offset and numel must be multiples of 16,"
+                         " numel >= 16, offset + numel <= 2**31")
+    dst = torch.empty_like(src)
+    z = torch.empty_like(src)
+    ws_bytes = _native.lib().tio_intensity_pass1_with_normals_workspace_bytes(offset, n)
+    workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=src.device)
+    table = _mt_table(src.device)
+    si = sj = sk = 0
+    if coarse is not None:
+        si, sj, sk = coarse.shape[2:]
+    with torch.cuda.device(src.device):
+        _native.call(
+            "tio_intensity_pass1_with_normals", _ptr(src), _ptr(dst), b, c, i, j, k,
+            _ptr(coarse), si, sj, sk, _ptr(bias_identity), int(bool(bias_divide)),
+            _ptr(taps), _ptr(radius), int(big_r), int(axes_mask),
+            int(seed) & 0xFFFFFFFF, offset, n, _ptr(z), _ptr(table), _ptr(workspace), ws_bytes,
+            _stream(src),
+        )
+    _count(4)
+    return dst, z
+
+
+def _intensity_fused_pass1_normals(src, coarse, bias_identity, bias_divide, taps, radius, big_r,
+                                   axes_mask, mean, std, keep, gamma, seed, offset) -> Tensor:
+    """`intensity_fused` with the exact-noise normals generated under its first pass: that pass
+    and the normals in one launch, then the J/K pass with noise and gamma at the store."""
+    first, z = intensity_pass1_with_normals(
+        src, seed, offset, coarse=coarse, bias_identity=bias_identity, bias_divide=bias_divide,
+        taps=taps, radius=radius, big_r=big_r, axes_mask=axes_mask)
+    return intensity_fused(first, taps=taps, radius=radius, big_r=big_r, axes_mask=axes_mask & 6,
+                           mean=mean, std=std, keep=keep, z=z, noise_mode=1, gamma=gamma)
 
 
 # ---- exact replay of torch's CPU randn stream (K4a) ---------------------------

@@ -192,7 +192,8 @@ def _blur_stage(ib, params, index: int = 0, whole: bool = False):
 def _noise_mode() -> str:
     """"exact" (default): the normals are the torch.randn draws of the recorded
     CPU-generator seed — the reference's stream (noise.py:166-178) — replayed on
-    the device by `ops.randn_mt19937` (host torch.randn only for ragged shapes).
+    the device by `ops.randn_mt19937`, or under the first pass of the fused chain
+    (host torch.randn only for ragged shapes).
     "philox": in-kernel counter-based normals — same distribution, other stream."""
     mode = os.environ.get("TIO_B200_NOISE", "exact").lower()
     if mode not in ("exact", "philox"):
@@ -258,10 +259,11 @@ def _noise_stage_factory(params):
 
     consumed = [0]  # words of the seed's stream used so far (across images and draws)
 
-    def draw(shape, device):
+    def draw(shape, device, defer=False):
         """Next ``prod(shape)`` normals of the stream: on the device when the
         position allows (multiples of 16), else with torch.randn on the host,
-        which the generator object keeps aligned with ``consumed``."""
+        which the generator object keeps aligned with ``consumed``.  ``defer``: a device draw
+        is returned as (seed, start) for `ops.intensity_fused` to make (``z_replay``)."""
         n = int(np.prod(shape))
         info = chunk_info()
         if info is None:
@@ -278,6 +280,8 @@ def _noise_stage_factory(params):
             ragged[0] = True  # torch's tail/scalar paths: stay on the host from here on
         consumed[0] += n_full + (16 if (n_full >= 16 and n_full % 16) else 0)
         if on_device:
+            if defer:
+                return (params["seed"], start), None
             return ops.randn_mt19937(params["seed"], start, n, device).view(shape), None
         # host path: fast-forward the CPU generator to `start` if the device path was used
         if host_state[0] != start:
@@ -309,8 +313,13 @@ def _noise_stage_factory(params):
             out["philox_seed"] = (int(params["seed"]) << 8) | (index & 0xFF)
             return out
         out["noise_mode"] = 1
-        z_dev, z_host = draw(shape, ib.data.device)
-        out["z" if z_dev is not None else "z_host"] = z_dev if z_dev is not None else z_host
+        # a single device draw is left to the fused call, which can make it under its first
+        # pass; the two draws of Rician noise are made here, one after the other
+        z_dev, z_host = draw(shape, ib.data.device, defer=not rician)
+        if z_host is not None:
+            out["z_host"] = z_host
+        else:
+            out["z" if rician else "z_replay"] = z_dev
         if rician:
             z_dev, z_host = draw(shape, ib.data.device)
             out["z2" if z_dev is not None else "z2_host"] = z_dev if z_dev is not None else z_host
