@@ -59,6 +59,10 @@ enum tio_interp { TIO_NEAREST = 0, TIO_LINEAR = 1, TIO_LABEL_PV = 2 };
 
 const char* tio_last_error(void);
 int tio_abi_version(void);
+/* Number of kernels the calling thread has launched through the library, counted at each launch
+ * (cudaMemsetAsync / cudaMemcpyAsync are not kernels and are not counted).  Thread-local, like
+ * tio_last_error(). */
+uint64_t tio_launch_count(void);
 
 /*
  * K1 — fused resample: affine matrix + trilinear control-point displacement +

@@ -65,3 +65,25 @@ def test_widened_entry_points_validate_before_launching():
         _native.call("tio_remap", p, p + 128, 4, 1, 1, 2, 2, 2, 6, 2, 2, 2, 0, 0, 2, None, None, None)
     # an empty upload is a no-op, not an error
     assert _native.lib().tio_upload(p, p + 128, 0, None) == 0
+
+
+def test_refused_calls_launch_nothing():
+    """tio_launch_count counts launches, not calls: entry points that fail their argument checks
+    (or have nothing to do) leave it where it was."""
+    import pytest
+
+    lib = _native.lib()
+    buf = ctypes.create_string_buffer(256)
+    p = ctypes.addressof(buf)
+    assert lib.tio_launch_count.restype is ctypes.c_uint64
+    before = lib.tio_launch_count()
+    assert isinstance(before, int) and before >= 0
+    with pytest.raises(RuntimeError, match="null"):
+        _native.call("tio_upload", None, None, 16, None)
+    with pytest.raises(RuntimeError, match="does not fit"):
+        _native.call("tio_crop_patches", p, p + 128, 4, 1, 4, 4, 4, 1, p, 8, 2, 2, None)
+    with pytest.raises(RuntimeError, match="null"):
+        _native.call("tio_intensity_fused", None, None, None, 1, 1, 1, 1, 16, None, 0, 0, 0, None, 0,
+                     None, None, 0, 0, None, None, None, None, None, 0, 0, 0, None, None)
+    assert lib.tio_upload(p, p + 128, 0, None) == 0
+    assert lib.tio_launch_count() == before

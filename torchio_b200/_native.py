@@ -14,7 +14,8 @@ from pathlib import Path
 
 LIB_PATH = Path(__file__).resolve().parent / "csrc" / "libtio_b200.so"
 
-# name -> argtypes  (every entry point of include/tio_b200.h)
+# name -> argtypes  (every entry point of include/tio_b200.h that returns int or size_t; lib() binds
+# tio_last_error and tio_launch_count itself)
 _SIGNATURES = {
     "tio_abi_version": [],
     "tio_resample": [c_void_p, c_void_p, c_int] + [c_int] * 8
@@ -95,6 +96,8 @@ def lib() -> ctypes.CDLL:
         handle = ctypes.CDLL(str(LIB_PATH))
         handle.tio_last_error.restype = c_char_p
         handle.tio_last_error.argtypes = []
+        handle.tio_launch_count.restype = c_uint64
+        handle.tio_launch_count.argtypes = []
         for name, argtypes in _SIGNATURES.items():
             fn = getattr(handle, name)
             fn.argtypes = argtypes
@@ -104,7 +107,7 @@ def lib() -> ctypes.CDLL:
 
 
 def exported_symbols() -> list[str]:
-    return ["tio_last_error", *_SIGNATURES]
+    return ["tio_last_error", "tio_launch_count", *_SIGNATURES]
 
 
 def call(name: str, *args) -> None:

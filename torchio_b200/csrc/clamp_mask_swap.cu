@@ -126,6 +126,7 @@ void launch_clamp(const void* src, void* dst, int64_t count, const void* lo, con
   const bool vectorised = (uintptr_t)src % (kVec * sizeof(S)) == 0 && (uintptr_t)dst % (kVec * sizeof(D)) == 0;
   clamp_kernel<S, D><<<(unsigned)grid_for(count / kVec + 1), kThreads, 0, st>>>(
       (const S*)src, (D*)dst, count, lo_v, hi_v, bounds, nan_value, vectorised ? 1 : 0);
+  launched();
 }
 
 // ---- mask ---------------------------------------------------------------------------------------
@@ -173,6 +174,7 @@ void launch_mask(const void* mask, int mask_channels, const void* keys, int n_ke
   mask_kernel<M, S, D><<<(unsigned)grid_for((int64_t)mask_channels * vox), kThreads, 0, st>>>(
       (const M*)mask, mask_channels, (const typename MaskKey<M>::type*)keys, n_keys, (const S*)src, (D*)dst, B,
       C, vox, host_value<D>(outside));
+  launched();
 }
 
 // in place, the image is never read: the outside value is stored as raw bytes of its width
@@ -340,6 +342,7 @@ int launch_swap(void* data, int B, int C, int I, int J, int K, int pi, int pj, i
   config.numAttrs = 1;
   TIO_CHECK_CUDA(cudaLaunchKernelEx(&config, swap_patches_kernel<T>, (T*)data, C, I, J, K, pi, pj, pk, list, steps,
                                     shared, (T*)stage));
+  launched();
   return 0;
 }
 

@@ -12,6 +12,11 @@ namespace tio {
 // thread-local error message (tio_last_error)
 void set_error(const char* fmt, ...);
 
+// thread-local count of kernels launched (tio_launch_count): every kernel launch in csrc/ is
+// followed by launched()
+extern thread_local uint64_t g_launches;
+inline void launched() { ++g_launches; }
+
 #define TIO_CHECK_ARG(cond, ...)       \
   do {                                 \
     if (!(cond)) {                     \

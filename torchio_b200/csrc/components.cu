@@ -352,14 +352,18 @@ void launch_components(const void* src, int B, const Shape& sh, const Select& se
   const dim3 tiles((unsigned)(((sh.I + kTI - 1) / kTI) * sh.tiles_j * sh.tiles_k), (unsigned)B);
   cc_local_kernel<T><<<tiles, kThreads, 0, st>>>((const T*)src, parent, count, flags, sh, sel, (const K*)keys,
                                                  neighbours);
+  launched();
   cc_merge_kernel<T><<<tiles, kThreads, 0, st>>>((const T*)src, parent, sh, neighbours);
+  launched();
   cc_compress_kernel<<<flat_grid(sh.vox, B), kFlatThreads, 0, st>>>(parent, count, sh.vox);
+  launched();
 }
 
 template <typename T>
 void launch_roots(const void* src, int B, unsigned long long vox, const unsigned* parent, void* values,
                   unsigned* n_values, cudaStream_t st) {
   cc_roots_kernel<T><<<flat_grid(vox, B), kFlatThreads, 0, st>>>((const T*)src, parent, vox, (T*)values, n_values);
+  launched();
 }
 
 template <typename T>
@@ -372,7 +376,9 @@ void launch_keep(void* data, int B, unsigned long long vox, const Select& sel, c
   const dim3 grid = flat_grid(vox, B);
   cc_winner_kernel<T><<<grid, kFlatThreads, 0, st>>>((const T*)data, parent, count, vox, sel, (const K*)keys, winner,
                                                      slots);
+  launched();
   cc_write_kernel<T><<<grid, kFlatThreads, 0, st>>>((T*)data, parent, vox, sel, (const K*)keys, winner, slots, value);
+  launched();
 }
 
 bool select_ok(int dtype, int mode, int n_keys, const void* keys) {

@@ -1,10 +1,12 @@
-// error.cu — thread-local error reporting for the C-ABI (tio_last_error).
+// error.cu — thread-local error reporting and launch count for the C-ABI (tio_last_error,
+// tio_launch_count).
 #include <stdarg.h>
 
 #include "common.cuh"
 
 namespace tio {
 static thread_local char g_error[512] = "";
+thread_local uint64_t g_launches = 0;
 
 void set_error(const char* fmt, ...) {
   va_list ap;
@@ -29,3 +31,4 @@ int num_sms() {
 
 extern "C" const char* tio_last_error(void) { return tio::g_error; }
 extern "C" int tio_abi_version(void) { return TIO_ABI_VERSION; }
+extern "C" uint64_t tio_launch_count(void) { return tio::g_launches; }

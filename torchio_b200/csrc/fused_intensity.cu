@@ -1066,6 +1066,7 @@ static int launch_jk(const float* src, float* dst, int B, int C, int I, int J, i
       cudaFuncSetAttribute(jk_kernel<RMAX, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     jk_kernel<RMAX, false><<<grid, 256, smem, st>>>(src, dst, B, C, I, J, K, bl, nz, gamma);
   }
+  launched();
   return 0;
 }
 
@@ -1091,6 +1092,7 @@ static int launch_march(const float* cur, float* out, int B, int C, int I, int J
       cudaFuncSetAttribute(march_kernel<VV, BB>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
                            (int)smem);                                                        \
     march_kernel<VV, BB><<<grid, block, smem, st>>>(cur, out, B, C, I, J, K, ib, bi, nz1, gamma1); \
+    launched();                                                                               \
   } while (0)
     if (vec && R <= F_R) {
       const size_t smem6 = (size_t)(16 + (ns + 3) / 4 * 4) * sizeof(float) + (size_t)M6_PF * 256 * 16;
@@ -1100,6 +1102,7 @@ static int launch_march(const float* cur, float* out, int B, int C, int I, int J
       cudaFuncSetAttribute(march6_kernel<BB, EE>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
                            (int)smem6);                                                        \
     march6_kernel<BB, EE><<<grid, block, smem6, st>>>(cur, out, B, C, I, J, K, ib, bi, nz1, gamma1); \
+    launched();                                                                                \
   } while (0)
       const bool epi = nz1.mode != 0 || gamma1 != nullptr;
       if (bi.coarse) { if (epi) TIO_LAUNCH_MARCH6(true, true); else TIO_LAUNCH_MARCH6(true, false); }
@@ -1145,6 +1148,7 @@ static int wide_impl(const float* src, float* dst, float* scratch, int B, int C,
       axis_kernel<true><<<grid, 256, smem, st>>>(cur, out, B, C, I, J, K, axes[s], bl, nz, gamma);
     else
       axis_kernel<false><<<grid, 256, smem, st>>>(cur, out, B, C, I, J, K, axes[s], bl, nz, gamma);
+    launched();
     cur = out;
   }
   TIO_CHECK_LAUNCH();
@@ -1214,6 +1218,7 @@ static int fused_impl(const float* src, float* dst, float* scratch, int B, int C
         cudaFuncSetAttribute(jk6_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)F_SMEM);
         jk6_kernel<false><<<grid, 256, F_SMEM, st>>>(tm, dst, B, C, I, J, K, bl, nz, gamma);
       }
+      launched();
     } else if (bl.R <= F_R) {
       launch_jk<6>(cur, dst, B, C, I, J, K, bl, nz, gamma, st);
     } else {
@@ -1315,6 +1320,7 @@ extern "C" int tio_intensity_pass1_with_normals(const float* src, float* dst, in
     pass1_normals_kernel<BB><<<grid, P1N_THREADS, smem, st>>>(src, dst, B, C, I, J, K, bl, bi, tile_counter, \
                                                               (const uint32_t*)workspace, q_lo, q_hi, seg,   \
                                                               offset, n, z);                                 \
+    launched();                                                                                              \
   } while (0)
   if (coarse) TIO_LAUNCH_P1N(true); else TIO_LAUNCH_P1N(false);
 #undef TIO_LAUNCH_P1N

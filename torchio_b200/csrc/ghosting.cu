@@ -167,7 +167,8 @@ extern "C" int tio_ghosting(void* data, int dtype, int B, int C, int I, int J, i
                                         (int)smem));                                                                \
     ghosting_kernel<T, false><<<grid, kThreads, smem, st>>>((T*)data, g, a, lines, S, plan, table, n_max, axis,   \
                                                             active, flags);                                         \
-  }
+  }                                                                                                                 \
+  launched();
     TIO_IMAGE_DISPATCH(dtype, "tio_ghosting", TIO_GHOST)
 #undef TIO_GHOST
     TIO_CHECK_LAUNCH();
@@ -176,7 +177,7 @@ extern "C" int tio_ghosting(void* data, int dtype, int B, int C, int I, int J, i
   const int64_t useful = (g.vox + kThreads - 1) / kThreads;
   if (parts > useful) parts = useful;
   const dim3 nan_grid((unsigned)parts, (unsigned)rows);
-#define TIO_NAN_ROWS(T) nan_rows_kernel<T><<<nan_grid, kThreads, 0, st>>>((T*)data, g.vox, flags)
+#define TIO_NAN_ROWS(T) nan_rows_kernel<T><<<nan_grid, kThreads, 0, st>>>((T*)data, g.vox, flags); launched()
   TIO_IMAGE_DISPATCH(dtype, "tio_ghosting", TIO_NAN_ROWS)
 #undef TIO_NAN_ROWS
   TIO_CHECK_LAUNCH();

@@ -197,6 +197,7 @@ void launch_interpolate(const void* src, void* dst, int volumes, int I, int J, i
   else
     interpolate_kernel<T, false><<<grid, kThreads, 0, st>>>((const T*)src, (T*)dst, I, J, K, OI, OJ, OK, idx, lam,
                                                             chunks);
+  launched();
 }
 
 template <typename T>
@@ -207,6 +208,7 @@ void launch_axis_resample(const void* src, void* dst, int B, int C, int I, int J
   const int64_t segments = (int64_t)B * C * I * J * ((K + V - 1) / V);
   axis_resample_kernel<T><<<grid_for(segments), kThreads, 0, st>>>(
       (const T*)src, (T*)dst, C, I, J, K, axis, lo, hi, w, L, linear, segments, vectorised ? 1 : 0);
+  launched();
 }
 
 }  // namespace

@@ -86,6 +86,7 @@ void launch_lut(const void* src, void* dst, int64_t count, const void* keys, con
   else if (n <= kSharedEntries) smem = (size_t)n * (sizeof(K) + sizeof(T));
   label_lut_kernel<T><<<(unsigned)blocks, kLutThreads, smem, st>>>(
       (const T*)src, (T*)dst, count, (const K*)keys, (const T*)values, n, identity, vectorised ? 1 : 0);
+  launched();
 }
 
 // ---- contour ------------------------------------------------------------------------------------
@@ -165,6 +166,7 @@ void launch_contour(const void* src, float* dst, int volumes, int I, int J, int 
                   (unsigned)volumes);
   label_contour_kernel<T><<<grid, kContourThreads, 0, st>>>((const T*)src, dst, I, J, K, tiles_k,
                                                             vectorised ? 1 : 0);
+  launched();
 }
 
 }  // namespace

@@ -82,6 +82,7 @@ static void launch_onehot(const void* src, int B, int64_t src_stride, int64_t vo
   if (blocks < 1) blocks = 1;
   onehot_kernel<T, kClasses><<<dim3((unsigned)blocks, B), 256, 0, st>>>(
       (const T*)src, src_stride, vox, (const typename LabelTable<T>::type*)labels, n, dst);
+  launched();
 }
 
 template <typename T>
@@ -92,6 +93,7 @@ static void launch_argmax(const float* sampled, int B, int n, int64_t vox, const
   if (blocks < 1) blocks = 1;
   label_argmax_kernel<T><<<dim3((unsigned)blocks, B), 256, 0, st>>>(
       sampled, n, vox, (const typename LabelTable<T>::type*)labels, pad, (T*)dst);
+  launched();
 }
 
 // ---- OneHot (transforms/label/one_hot.py:58-97) -----------------------------------------------
@@ -239,8 +241,11 @@ extern "C" int tio_label_range(const void* src, int dtype, int B, int C, int64_t
   cudaStream_t st = (cudaStream_t)stream;
   long long* out = (long long*)range;
   label_range_init<<<1, 1, 0, st>>>(out);
+  launched();
   const dim3 grid((unsigned)((stream_blocks(vox) + B - 1) / B), B);
-#define TIO_RANGE(T) label_range_kernel<T><<<grid, 256, 0, st>>>((const T*)src, (int64_t)C * vox, vox, out)
+#define TIO_RANGE(T) \
+  label_range_kernel<T><<<grid, 256, 0, st>>>((const T*)src, (int64_t)C * vox, vox, out); \
+  launched()
   TIO_LABEL_DISPATCH(dtype, "tio_label_range", TIO_RANGE)
 #undef TIO_RANGE
   TIO_CHECK_LAUNCH();
@@ -255,7 +260,9 @@ extern "C" int tio_channel_argmax(const void* src, int dtype, int B, int C, int6
   cudaStream_t st = (cudaStream_t)stream;
   const int vectorised = vox % 4 == 0 && (uintptr_t)src % (4 * 8) == 0 && (uintptr_t)dst % 16 == 0;
   const dim3 grid((unsigned)stream_blocks(vectorised ? vox / 4 : vox), B);
-#define TIO_ARGMAX(T) channel_argmax_kernel<T><<<grid, 256, 0, st>>>((const T*)src, C, vox, vectorised, dst)
+#define TIO_ARGMAX(T) \
+  channel_argmax_kernel<T><<<grid, 256, 0, st>>>((const T*)src, C, vox, vectorised, dst); \
+  launched()
   TIO_LABEL_DISPATCH(dtype, "tio_channel_argmax", TIO_ARGMAX)
 #undef TIO_ARGMAX
   TIO_CHECK_LAUNCH();

@@ -132,6 +132,7 @@ void launch(const void* labels, int C, uint32_t vox, uint32_t N, const long long
   const size_t smem = (size_t)n * 16 + (kByteLabels<T> ? kThreads * sizeof(int) : 0);
   labels_to_image_kernel<T><<<grid, kThreads, smem, st>>>((const T*)labels, C, vox, N, values, n, mean, std,
                                                           offs, seed, iters, out);
+  launched();
 }
 
 }  // namespace

@@ -126,6 +126,7 @@ int mt_start_states(uint64_t seed, uint64_t offset, uint64_t n, const void* tabl
   uint32_t* states = (uint32_t*)workspace;
   const uint16_t* polys = (const uint16_t*)((const char*)table + tio_mt::kHeaderBytes);
   mt_seed_kernel<<<1, 32, 0, st>>>((uint32_t)seed, states);
+  launched();
   const size_t jump_smem = (size_t)(MT_OFFS + 2048) * 4;
   cudaFuncSetAttribute(mt_jump_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)jump_smem);
   const int m_lo = (int)(q_lo / S2), m_hi = (int)((q_hi - 1) / S2);
@@ -137,8 +138,10 @@ int mt_start_states(uint64_t seed, uint64_t offset, uint64_t n, const void* tabl
     cudaMemset2DAsync(states + (size_t)m_first * S2 * MT_N, pitch, 0, MT_N * 4, m_hi - m_first + 1, st);
     mt_jump_kernel<<<(m_hi - m_first + 1) * kCoarseParts, 640, jump_smem, st>>>(states, polys, stride, m_first,
                                                                              S2, 0, kCoarseParts);
+    launched();
   }
   mt_jump_kernel<<<(unsigned)(q_hi - q_lo), 640, jump_smem, st>>>(states, polys, stride, (int)q_lo, S2, 1, 1);
+  launched();
   *q_lo_out = (int)q_lo;
   *q_hi_out = (int)q_hi;
   return 0;
@@ -165,6 +168,7 @@ extern "C" int tio_randn_mt19937(uint64_t seed, uint64_t offset, uint64_t n, flo
     return rc;
   mt_normal_kernel<<<(unsigned)(q_hi - q_lo), MT_THREADS, 0, st>>>((const uint32_t*)workspace, q_lo, MT_L, offset,
                                                                    n, z);
+  launched();
   TIO_CHECK_LAUNCH();
   return 0;
 }

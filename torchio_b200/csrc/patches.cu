@@ -70,12 +70,14 @@ static void launch_crop(const void* src, void* dst, int C, int I, int J, int K, 
     const long long units = rows * (pk / V);
     const unsigned blocks = (unsigned)((units + 255) / 256);
     crop_patches_vec_kernel<T><<<blocks, 256, 0, st>>>((const T*)src, (T*)dst, C, I, J, K, units, corners, pi, pj, pk);
+    launched();
     return;
   }
   const int tx = pk >= 128 ? 128 : (pk >= 64 ? 64 : 32);
   dim3 block(tx, 256 / tx);
   const unsigned blocks = (unsigned)((rows + block.y - 1) / block.y);
   crop_patches_kernel<T><<<blocks, block, 0, st>>>((const T*)src, (T*)dst, C, I, J, K, n, corners, pi, pj, pk);
+  launched();
 }
 
 }  // namespace tio
@@ -221,6 +223,7 @@ static void launch_remap(const void* src, void* dst, int B, int C, int I, int J,
     const long long units = rows * (OK / V);
     remap_vec_kernel<T><<<(unsigned)((units + 255) / 256), 256, 0, st>>>(
         (const T*)src, (T*)dst, B, C, I, J, K, OI, OJ, OK, oi, oj, ok, mode, fill, flip, units);
+    launched();
     return;
   }
   const int tx = OK >= 128 ? 128 : (OK >= 64 ? 64 : 32);
@@ -228,6 +231,7 @@ static void launch_remap(const void* src, void* dst, int B, int C, int I, int J,
   const unsigned blocks = (unsigned)((rows + block.y - 1) / block.y);
   remap_kernel<T><<<blocks, block, 0, st>>>((const T*)src, (T*)dst, B, C, I, J, K, OI, OJ, OK, oi, oj, ok,
                                             mode, fill, flip);
+  launched();
 }
 
 }  // namespace tio

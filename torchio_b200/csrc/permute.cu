@@ -172,6 +172,7 @@ static void launch_tile(const void* src, void* dst, TileGeometry g, long long bl
   g.word_load = g.word_load && g.K % P == 0 && ((uintptr_t)src % sizeof(W)) == 0;
   g.word_store = g.word_store && g.n_a % P == 0 && ((uintptr_t)dst % sizeof(W)) == 0;
   permute_tile_kernel<T, W><<<(unsigned)blocks, 256, 0, st>>>((const T*)src, (T*)dst, g);
+  launched();
 }
 
 template <typename T>
@@ -182,12 +183,14 @@ static void launch_ij(const void* src, void* dst, int B, int C, int I, int J, in
     const long long units = rows * (K / V);
     permute_ij_vec_kernel<T><<<(unsigned)((units + 255) / 256), 256, 0, st>>>((const T*)src, (T*)dst, I, J, K,
                                                                               flips, units);
+    launched();
     return;
   }
   const int tx = K >= 128 ? 128 : (K >= 64 ? 64 : 32);
   dim3 block(tx, 256 / tx);
   permute_ij_kernel<T><<<(unsigned)((rows + block.y - 1) / block.y), block, 0, st>>>((const T*)src, (T*)dst, I, J,
                                                                                       K, flips, rows);
+  launched();
 }
 
 static int tile_edge(int elem_bytes) { return elem_bytes < 4 ? 32 * (4 / elem_bytes) : 32; }

@@ -69,6 +69,7 @@ static int launch_fill(const ResampleArgs& a, dim3 grid, dim3 block, size_t smem
     resample_kernel<T, MODE, HAS_CP, true><<<grid, block, smem, st>>>(a);
   else
     resample_kernel<T, MODE, HAS_CP, false><<<grid, block, smem, st>>>(a);
+  launched();
   return 0;
 }
 
@@ -98,6 +99,7 @@ static int launch_typed(const ResampleArgs& a, int mode, cudaStream_t st) {
     } else {
       resample_kernel<T, TIO_LABEL_PV, false, true><<<grid, block, smem, st>>>(a);
     }
+    launched();
     return 0;
   }
   if (mode == TIO_NEAREST) {
@@ -225,6 +227,7 @@ extern "C" int tio_min_sample0(const float* src, int C, int64_t n, float* fill, 
   TIO_CHECK_ARG(src && fill && C > 0 && n > 0, "tio_min_sample0: bad arguments");
   cudaStream_t st = (cudaStream_t)stream;
   min_init_kernel<<<(C + 31) / 32, 32, 0, st>>>(fill, C);
+  launched();
   const bool vec = (((uintptr_t)src & 15) == 0) && ((n & 3) == 0);
   int64_t work = vec ? (n >> 2) : n;
   int blocks = (int)((work + 255) / 256);
@@ -234,6 +237,7 @@ extern "C" int tio_min_sample0(const float* src, int C, int64_t n, float* fill, 
     min_kernel<true><<<dim3(blocks, C), 256, 0, st>>>(src, n, fill);
   else
     min_kernel<false><<<dim3(blocks, C), 256, 0, st>>>(src, n, fill);
+  launched();
   TIO_CHECK_LAUNCH();
   return 0;
 }

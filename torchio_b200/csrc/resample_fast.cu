@@ -457,6 +457,7 @@ static void launch_fast_cp(const CUtensorMap& tm, const CUtensorMap& tms, const 
                          (int)smem);
     resample_fast_kernel<BOX, HAS_CP, false><<<grid, 256, smem, st>>>(tm, tms, a, ta, records);
   }
+  launched();
 }
 
 template <int BOX>

@@ -564,6 +564,7 @@ static bool fastdiv_admitted(float d, cudaStream_t st) {
   if (cudaMalloc(&bad, 8) == cudaSuccess) {
     cudaMemsetAsync(bad, 0, 8, st);
     verify_fastdiv_kernel<<<num_sms() * 16, 256, 0, st>>>(d, (float)(1.0 / (double)d), bad);
+    launched();
     unsigned long long host = 1;
     if (cudaMemcpyAsync(&host, bad, 8, cudaMemcpyDeviceToHost, st) == cudaSuccess &&
         cudaStreamSynchronize(st) == cudaSuccess)
@@ -587,6 +588,7 @@ static void launch_tile(const CUtensorMap& tm, const ResampleArgs& a, const Tile
                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     resample_tile_kernel<BOX, T, MODE, HAS_CP, false, FASTDIV><<<grid, 256, smem, st>>>(tm, a, ta, records);
   }
+  launched();
 }
 
 template <int BOX>
@@ -719,6 +721,7 @@ int launch_resample_tile(const ResampleArgs& a, int dtype, int mode, bool exact_
   }
   if (a.cp) tile_bounds_kernel<true><<<bounds_blocks, 128, 0, st>>>(a, box, kalign, bk, box_s, bk_s, records);
   else tile_bounds_kernel<false><<<bounds_blocks, 128, 0, st>>>(a, box, kalign, bk, box_s, bk_s, records);
+  launched();
   const size_t smem = ((size_t)box * box * bk * esize + 15) / 16 * 16 + kAuxFloats * sizeof(float);
   if (mode == TIO_LABEL_PV) {
     if (dtype == TIO_U8) launch_label_pv<uint8_t>(box, tm, a, ta, grid, smem, records, st);

@@ -334,7 +334,8 @@ extern "C" int tio_spike_stats(const void* src, int dtype, int B, int C, int64_t
   const dim3 grid((unsigned)stats_parts(rows, vox), (unsigned)rows);
 #define TIO_STATS(T)                                                                                     \
   stats_kernel<T><<<grid, kThreads, 0, st>>>((const T*)src, C, vox, intensity, sum, flags, part_sum, \
-                                             part_flags, tickets)
+                                             part_flags, tickets);                                   \
+  launched()
   TIO_IMAGE_DISPATCH(dtype, "tio_spike_stats", TIO_STATS)
 #undef TIO_STATS
   TIO_CHECK_LAUNCH();
@@ -374,13 +375,16 @@ extern "C" int tio_spectrum_peak(const void* src, int dtype, int B, int C, int I
   TIO_CHECK_CUDA(cudaFuncSetAttribute(fft_k_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sk)); \
   fft_k_kernel<T><<<dim3((unsigned)k_blocks, (unsigned)n), kThreads, sk, st>>>((const T*)src, g, row0, lk,    \
                                                                                line_stride(K), pk, intensity, \
-                                                                               flags, ws)
+                                                                               flags, ws);                    \
+  launched()
     TIO_IMAGE_DISPATCH(dtype, "tio_spectrum_peak", TIO_FFT_K)
 #undef TIO_FFT_K
     fft_strided_kernel<<<dim3((unsigned)j_blocks, (unsigned)n), kThreads, sj, st>>>(
         g, row0, lj, line_stride(J), pj, 0, intensity, flags, ws, peak);
+    launched();
     fft_strided_kernel<<<dim3((unsigned)i_blocks, (unsigned)n), kThreads, si, st>>>(
         g, row0, li, line_stride(I), pi, 1, intensity, flags, ws, peak);
+    launched();
     TIO_CHECK_LAUNCH();
   }
   return 0;
@@ -412,12 +416,14 @@ extern "C" int tio_spike(void* data, int dtype, int B, int C, int I, int J, int 
                                        ? (table_entries + kThreads - 1) / kThreads
                                        : 4096),
                         kThreads, 0, st>>>((const int4*)spikes, B, S, I, J, K, intensity, (float2*)tables);
+  launched();
   const dim3 grid((unsigned)parts, (unsigned)rows);
 #define TIO_SPIKE(T)                                                                                        \
   if (in_smem)                                                                                              \
     TIO_CHECK_CUDA(cudaFuncSetAttribute(spike_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
   spike_kernel<T><<<grid, kThreads, in_smem ? smem : 0, st>>>((T*)data, g, (const int4*)spikes, S, intensity, sum, \
-                                                              flags, peak, (const float2*)tables, in_smem)
+                                                              flags, peak, (const float2*)tables, in_smem); \
+  launched()
   TIO_IMAGE_DISPATCH(dtype, "tio_spike", TIO_SPIKE)
 #undef TIO_SPIKE
   TIO_CHECK_LAUNCH();

@@ -424,6 +424,7 @@ extern "C" int tio_moments(const float* src, const uint8_t* mask, int64_t n, dou
   if (blocks > num_sms() * 8) blocks = num_sms() * 8;
   if (blocks < 1) blocks = 1;
   moments_kernel<<<blocks, 256, 0, st>>>(src, mask, n, out3);
+  launched();
   TIO_CHECK_LAUNCH();
   return 0;
 }
@@ -469,6 +470,7 @@ int launch_select_hist(const void* src, const uint8_t* mask, int B, int64_t per_
   if (bx < 1) bx = 1;
   kernel<<<dim3(bx, B), kSelectThreads, smem, st>>>((const T*)src, mask, per_elem, l.state,
                                                    LEVEL == 0 ? l.hist0 : l.hist, l.slots);
+  launched();
   TIO_CHECK_LAUNCH();
   return 0;
 }
@@ -479,6 +481,7 @@ int run_select(const void* src, const uint8_t* mask, int B, int64_t per_elem, co
                cudaStream_t st) {
   int rc;
   select_reset_kernel<<<B, 1, 0, st>>>(l.state);
+  launched();
   TIO_CHECK_CUDA(cudaMemsetAsync(l.hist0, 0, (size_t)B * kBins0 * sizeof(unsigned), st));
   if ((rc = launch_select_hist<T, 0>(src, mask, B, per_elem, l, st))) return rc;
   const size_t hbytes = (size_t)B * l.slots * kBins1 * sizeof(unsigned);
@@ -489,14 +492,17 @@ int run_select(const void* src, const uint8_t* mask, int B, int64_t per_elem, co
     for (int j = 0; j < kQuantPerRound; ++j) rq.q[j] = j < rq.nq ? q_host[first + j] : 0.0;
     select_scan_kernel<0><<<B, kSelectThreads, 0, st>>>(l.state, l.hist0, l.hist, l.slots, rq, per_elem,
                                                          mask != nullptr, m, values, weights, count, has_nan);
+    launched();
     TIO_CHECK_CUDA(cudaMemsetAsync(l.hist, 0, hbytes, st));
     if ((rc = launch_select_hist<T, 1>(src, mask, B, per_elem, l, st))) return rc;
     select_scan_kernel<1><<<B, kSelectThreads, 0, st>>>(l.state, l.hist0, l.hist, l.slots, rq, per_elem,
                                                          mask != nullptr, m, values, weights, count, has_nan);
+    launched();
     TIO_CHECK_CUDA(cudaMemsetAsync(l.hist, 0, hbytes, st));
     if ((rc = launch_select_hist<T, 2>(src, mask, B, per_elem, l, st))) return rc;
     select_scan_kernel<2><<<B, kSelectThreads, 0, st>>>(l.state, l.hist0, l.hist, l.slots, rq, per_elem,
                                                          mask != nullptr, m, values, weights, count, has_nan);
+    launched();
     TIO_CHECK_LAUNCH();
   }
   return 0;
@@ -543,6 +549,7 @@ extern "C" int tio_histogram_tables(const float* values, const double* weights, 
   TIO_CHECK_ARG(values && weights && landmarks && tables, "tio_histogram_tables: null pointer");
   TIO_CHECK_ARG(B >= 1 && m >= 2, "tio_histogram_tables: need B >= 1 and at least 2 landmarks");
   histogram_tables_kernel<<<B, 32, 0, (cudaStream_t)stream>>>(values, weights, has_nan, landmarks, m, tables);
+  launched();
   TIO_CHECK_LAUNCH();
   return 0;
 }
@@ -562,6 +569,7 @@ extern "C" int tio_histogram_map(const void* src, void* dst, int dtype, int B, i
     if (bx > cap) bx = cap;                                                                         \
     histogram_map_kernel<T><<<dim3((unsigned)bx, B), 256, smem, st>>>((const T*)src, (T*)dst, per_elem, \
                                                                       tables, m);                   \
+    launched();                                                                                     \
   }
   TIO_IMAGE_DISPATCH(dtype, "tio_histogram_map", TIO_MAP)
 #undef TIO_MAP
@@ -584,6 +592,7 @@ extern "C" int tio_rescale(const float* src, float* dst, int B, int64_t per_elem
   dim3 grid(bx, B);
   if (vec) rescale_kernel<4><<<grid, 256, 0, st>>>(src, dst, per_elem, lo, hi, sub, div, mul, add, keep, flags);
   else rescale_kernel<1><<<grid, 256, 0, st>>>(src, dst, per_elem, lo, hi, sub, div, mul, add, keep, flags);
+  launched();
   TIO_CHECK_LAUNCH();
   return 0;
 }

@@ -25,6 +25,7 @@ extern "C" int tio_upload(const void* host_pinned, void* dst_device, size_t byte
   const unsigned blocks = (unsigned)((items + 255) / 256);
   tio::upload_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>((const uint8_t*)host_pinned,
                                                              (uint8_t*)dst_device, bytes);
+  tio::launched();
   TIO_CHECK_LAUNCH();
   return 0;
 }

@@ -25,16 +25,10 @@ DTYPE_CODES = {
 NEAREST, LINEAR, LABEL_PV = 0, 1, 2
 FLAG_PASSTHROUGH, FLAG_ELASTIC = 1, 2
 
-_counter = threading.local()
-
-
 def launches() -> int:
-    """Number of kernels this thread has launched through the library."""
-    return getattr(_counter, "n", 0)
-
-
-def _count(n: int) -> None:
-    _counter.n = getattr(_counter, "n", 0) + n
+    """Number of kernels this thread has launched through the library, counted by the library at
+    each launch (`tio_launch_count`)."""
+    return _native.lib().tio_launch_count()
 
 
 def _stream(t: Tensor) -> int:
@@ -140,7 +134,6 @@ def upload(device: torch.device, *arrays):
         dev = torch.empty(offset, dtype=torch.uint8, device=device)
         _native.call("tio_upload", stage.data_ptr(), dev.data_ptr(), offset,
                      torch.cuda.current_stream(dev.device).cuda_stream)
-        _count(1)
         _ring.release(slot, torch.device(device))
     else:
         dev = stage.to(device, non_blocking=True)
@@ -214,7 +207,6 @@ def resample(
             int(mode) | (EXACT_COORDS if (_exact_default if exact_coords is None else exact_coords) else 0),
             _ptr(fill), int(box_hint), _ptr(workspace), ws_bytes, _stream(src),
         )
-    _count(2 if workspace is not None else 1)
     return dst
 
 
@@ -236,7 +228,6 @@ def onehot(src: Tensor, labels: Tensor) -> Tensor:
     with torch.cuda.device(src.device):
         _native.call("tio_onehot", _ptr(src), DTYPE_CODES[src.dtype], b, vox, _ptr(table), n, _ptr(dst),
                      _stream(src))
-    _count(1)
     return dst
 
 
@@ -254,7 +245,6 @@ def label_argmax(sampled: Tensor, labels: Tensor, pad_label: float, dtype: torch
     with torch.cuda.device(sampled.device):
         _native.call("tio_label_argmax", _ptr(sampled), b, n, vox, _ptr(table), float(pad_label), _ptr(dst),
                      DTYPE_CODES[dtype], _stream(sampled))
-    _count(1)
     return dst
 
 
@@ -268,7 +258,6 @@ def min_sample0(src: Tensor) -> Tensor:
     fill = torch.empty(c, dtype=torch.float32, device=src.device)
     with torch.cuda.device(src.device):
         _native.call("tio_min_sample0", _ptr(src), c, n, _ptr(fill), _stream(src))
-    _count(2)
     return fill
 
 
@@ -302,7 +291,6 @@ def crop_patches(volume: Tensor, corners, size, out: Tensor | None = None) -> Te
             "tio_crop_patches", _ptr(volume), _ptr(dst), volume.element_size(), c, i, j, k, n,
             _ptr(corners_d), pi, pj, pk, _stream(volume),
         )
-    _count(1)
     return dst
 
 
@@ -334,7 +322,6 @@ def remap(src: Tensor, out_shape, offsets, *, mode: str = "constant", fill=0, fl
             int(offsets[0]), int(offsets[1]), int(offsets[2]), PAD_MODES[mode],
             fill_host.data_ptr(), _ptr(flip), _stream(src),
         )
-    _count(1)
     return dst
 
 
@@ -363,7 +350,6 @@ def permute(src: Tensor, perm, flip_bits: int = 0) -> Tensor:
     with torch.cuda.device(src.device):
         _native.call("tio_permute", _ptr(src), _ptr(dst), src.element_size(), b, c, i, j, k, *perm, flip_bits,
                      _stream(src))
-    _count(1)
     return dst
 
 
@@ -380,21 +366,12 @@ def blur(src: Tensor, taps: Tensor, radius: Tensor, big_r: int, axes_mask: int,
             "tio_blur", _ptr(src), _ptr(dst), _ptr(scratch), b, c, i, j, k, _ptr(taps),
             _ptr(radius), int(big_r), int(axes_mask), _ptr(identity), _stream(src),
         )
-    _count(_fused_launches(axes_mask, False, big_r))
     return dst
 
 
 #: Tables with a larger radius run one launch per blurred axis (after the bias pass), through
 #: a scratch buffer whatever the axes.
 WIDE_R = 16
-
-
-def _fused_launches(axes_mask: int, has_bias: bool, big_r: int = 0) -> int:
-    if axes_mask & 7 and big_r > WIDE_R:
-        return bin(axes_mask & 7).count("1") + int(has_bias)
-    jk = bool(axes_mask & 6)
-    march = (not jk) or bool(axes_mask & 1) or has_bias
-    return int(jk) + int(march)
 
 
 def moments(values: Tensor, mask: Tensor | None = None) -> tuple[float, float, float]:
@@ -407,7 +384,6 @@ def moments(values: Tensor, mask: Tensor | None = None) -> tuple[float, float, f
     out = torch.empty(3, dtype=torch.float64, device=values.device)
     with torch.cuda.device(values.device):
         _native.call("tio_moments", _ptr(values), _ptr(m8), values.numel(), _ptr(out), _stream(values))
-    _count(1)
     s, ss, n = out.tolist()
     return s, ss, n
 
@@ -429,7 +405,6 @@ def quantile_neighbours(values: Tensor, qs, mask: Tensor | None = None):
     with torch.cuda.device(dev):
         _native.call("tio_quantiles", _ptr(values), _ptr(m8), values.numel(), qs.ctypes.data, m, _ptr(vals),
                      _ptr(out), out[m:].data_ptr(), _ptr(ws), ws_bytes, _stream(values))
-    _count(7)
     host = out.tolist()
     return vals.tolist(), host[:m], int(host[m])
 
@@ -459,7 +434,6 @@ def quantiles_batched(values: Tensor, qs, mask: Tensor | None = None):
         _native.call("tio_quantiles_batched", _ptr(values), RESOLUTION_DTYPE_CODES[values.dtype], _ptr(m8), b,
                      per_elem, qs.ctypes.data, m, _ptr(vals), _ptr(weights), _ptr(count), _ptr(has_nan), _ptr(ws),
                      ws_bytes, _stream(values))
-    _count(2 + 5 * ((m + 12) // 13))
     return vals, weights, count, has_nan
 
 
@@ -473,7 +447,6 @@ def histogram_tables(values: Tensor, weights: Tensor, has_nan: Tensor, landmarks
     with torch.cuda.device(values.device):
         _native.call("tio_histogram_tables", _ptr(values), _ptr(weights), _ptr(has_nan), _ptr(landmarks), b, m,
                      _ptr(tables), _stream(values))
-    _count(1)
     return tables
 
 
@@ -491,7 +464,6 @@ def histogram_map(data: Tensor, tables: Tensor, m: int) -> None:
     with torch.cuda.device(data.device):
         _native.call("tio_histogram_map", _ptr(data), _ptr(data), RESOLUTION_DTYPE_CODES[data.dtype], data.shape[0],
                      data[0].numel(), _ptr(tables), int(m), _stream(data))
-    _count(1)
 
 
 def rescale(src: Tensor, *, lo: float | None = None, hi: float | None = None, sub=None, div=None, mul=None,
@@ -518,7 +490,6 @@ def rescale(src: Tensor, *, lo: float | None = None, hi: float | None = None, su
         _native.call("tio_rescale", _ptr(src), _ptr(dst), b, src[0].numel(),
                      float(lo if lo is not None else 0.0), float(hi if hi is not None else 0.0),
                      _ptr(sub_d), _ptr(div_d), _ptr(mul_d), _ptr(add_d), _ptr(keep_d), flags, _stream(src))
-    _count(2)
     return dst
 
 
@@ -571,7 +542,6 @@ def intensity_fused(
             int(philox_seed) & (2**64 - 1), int(noise_mode), int(bool(rician)),
             _ptr(gamma), _stream(src),
         )
-    _count(_fused_launches(axes_mask if taps is not None else 0, coarse is not None, big_r))
     return dst
 
 
@@ -607,7 +577,6 @@ def intensity_pass1_with_normals(
             int(seed) & 0xFFFFFFFF, offset, n, _ptr(z), _ptr(table), _ptr(workspace), ws_bytes,
             _stream(src),
         )
-    _count(4)
     return dst, z
 
 
@@ -688,7 +657,6 @@ def randn_mt19937(seed: int, offset: int, n: int, device, out: Tensor | None = N
     with torch.cuda.device(device):
         _native.call("tio_randn_mt19937", int(seed) & 0xFFFFFFFF, offset, n, _ptr(z), _ptr(table),
                      _ptr(workspace), ws_bytes, torch.cuda.current_stream(device).cuda_stream)
-    _count(4)
     return z
 
 
@@ -751,7 +719,6 @@ def labels_to_image(labels: Tensor, label_values, means, stds, draw=None) -> Ten
         _native.call("tio_labels_to_image", _ptr(labels), DTYPE_CODES[labels.dtype], c, b, vox, _ptr(values_d), n,
                      _ptr(mean_d), _ptr(std_d), _ptr(offsets_d), seed & (2**64 - 1), grid_x, _ptr(out),
                      _stream(labels))
-    _count(2 if n else 1)
     return out
 
 
@@ -778,7 +745,6 @@ def label_lut(src: Tensor, keys: np.ndarray, values: np.ndarray, *, identity: bo
     with torch.cuda.device(src.device):
         _native.call("tio_label_lut", _ptr(src), _ptr(dst), DTYPE_CODES[src.dtype], src.numel(), _ptr(keys_d),
                      _ptr(values_d), n, int(bool(identity)), _stream(src))
-    _count(2 if n else 1)
     return dst
 
 
@@ -792,7 +758,6 @@ def label_contour(src: Tensor) -> Tensor:
         with torch.cuda.device(src.device):
             _native.call("tio_label_contour", _ptr(src), DTYPE_CODES[src.dtype], b * c, i, j, k, _ptr(dst),
                          _stream(src))
-        _count(1)
     return dst
 
 
@@ -805,7 +770,6 @@ def label_range(src: Tensor) -> tuple[int, int]:
     with torch.cuda.device(src.device):
         _native.call("tio_label_range", _ptr(src), DTYPE_CODES[src.dtype], b, c, src[0, 0].numel(), _ptr(out),
                      _stream(src))
-    _count(2)
     lo, hi = out.tolist()
     return lo, hi
 
@@ -819,7 +783,6 @@ def onehot_classes(src: Tensor, num_classes: int) -> Tensor:
     with torch.cuda.device(src.device):
         _native.call("tio_onehot_classes", _ptr(src), DTYPE_CODES[src.dtype], b, c, src[0, 0].numel(),
                      int(num_classes), _ptr(dst), _stream(src))
-    _count(1)
     return dst
 
 
@@ -832,7 +795,6 @@ def channel_argmax(src: Tensor) -> Tensor:
     with torch.cuda.device(src.device):
         _native.call("tio_channel_argmax", _ptr(src), DTYPE_CODES[src.dtype], b, c, src[0, 0].numel(), _ptr(dst),
                      _stream(src))
-    _count(1)
     return dst
 
 
@@ -865,7 +827,6 @@ def interpolate(src: Tensor, out_shape, idx: np.ndarray, lam: np.ndarray | None)
         with torch.cuda.device(src.device):
             _native.call("tio_interpolate", _ptr(src), _ptr(dst), RESOLUTION_DTYPE_CODES[src.dtype], b * c, i, j, k, oi, oj,
                          ok, _ptr(idx_d), _ptr(lam_d), int(lam is not None), _stream(src))
-        _count(1)
     return dst
 
 
@@ -886,7 +847,6 @@ def axis_resample(src: Tensor, axis: np.ndarray, lo: np.ndarray, hi: np.ndarray,
             _native.call("tio_axis_resample", _ptr(src), _ptr(dst), RESOLUTION_DTYPE_CODES[src.dtype], b, c, i, j, k,
                          _ptr(axis_d), _ptr(lo_d), _ptr(hi_d), _ptr(w_d), int(lo.shape[1]), int(bool(linear)),
                          _stream(src))
-        _count(1)
     return dst
 
 
@@ -917,7 +877,6 @@ def clamp(src: Tensor, lo: Tensor | None, hi: Tensor | None) -> Tensor:
     with torch.cuda.device(src.device):
         _native.call("tio_clamp", _ptr(src), _ptr(dst), RESOLUTION_DTYPE_CODES[src.dtype],
                      RESOLUTION_DTYPE_CODES[dst.dtype], src.numel(), lo_ptr, hi_ptr, _stream(src))
-    _count(1)
     del lo_keep, hi_keep
     return dst
 
@@ -952,7 +911,6 @@ def mask(data: Tensor, mask: Tensor, keys: np.ndarray | None, outside: Tensor) -
             _native.call("tio_mask", _ptr(mask), DTYPE_CODES[mask.dtype], mask.shape[0], _ptr(keys_d), n,
                          _ptr(data), RESOLUTION_DTYPE_CODES[data.dtype], _ptr(dst), RESOLUTION_DTYPE_CODES[dst.dtype],
                          b, c, data[0, 0].numel(), outside_ptr, _stream(data))
-        _count(2 if n > 0 else 1)
     del keep
     return dst
 
@@ -981,7 +939,6 @@ def swap_patches(data: Tensor, swaps: np.ndarray, patch_size) -> None:
     with torch.cuda.device(data.device):
         _native.call("tio_swap_patches", _ptr(data), data.element_size(), b, c, i, j, k, pi, pj, pk,
                      swaps.ctypes.data, lists, steps, _ptr(device_list), _ptr(stage), _stream(data))
-    _count(2)
 
 
 # ---- KeepLargestComponent (label/keep_largest.py) -----------------------------------------------
@@ -1048,13 +1005,11 @@ def keep_largest(data: Tensor, labels, background_label, fully_connected: bool) 
     with torch.cuda.device(dev):
         _native.call("tio_components", _ptr(data), code, b, i, j, k, mode, _ptr(keys_d), n, key, has_key,
                      int(bool(fully_connected)), _ptr(roots), _ptr(count), _ptr(flags), _stream(data))
-        _count(3)
         if mode == KEEP_SEARCH and b * vox:
             values = torch.empty(b * vox, dtype=dtype, device=dev)
             n_values = torch.empty(1, dtype=torch.int32, device=dev)
             _native.call("tio_component_roots", _ptr(data), code, b, vox, _ptr(roots), _ptr(values),
                          _ptr(n_values), _stream(data))
-            _count(1)
             found = values[:int(n_values.item())]  # the one read-back: the distinct labels present
             keys_d = torch.unique(found).to(torch.float32 if dtype == torch.float32 else torch.int64).contiguous()
             n = int(keys_d.numel())
@@ -1075,7 +1030,6 @@ def keep_largest(data: Tensor, labels, background_label, fully_connected: bool) 
     with torch.cuda.device(dev):
         _native.call("tio_keep_largest", _ptr(data), code, b, vox, mode, _ptr(keys_d), n, key, has_key, _ptr(roots),
                      _ptr(count), _ptr(winner), fill_ptr, _stream(data))
-    _count(2)
     del keep
     return data, roots
 
@@ -1119,7 +1073,6 @@ def spike(data: Tensor, spikes: np.ndarray, intensity: np.ndarray) -> Tensor:
         _native.call("tio_spike", _ptr(data), RESOLUTION_DTYPE_CODES[data.dtype], b, c, i, j, k, _ptr(spikes_d), s,
                      _ptr(intensity_d), _ptr(total), _ptr(flags), _ptr(peak), _ptr(tables), tables_bytes,
                      _stream(data))
-    _count(2)
     return data
 
 
@@ -1134,7 +1087,6 @@ def spike_stats(data: Tensor, intensity: Tensor) -> tuple[Tensor, Tensor]:
     with torch.cuda.device(data.device):
         _native.call("tio_spike_stats", _ptr(data), RESOLUTION_DTYPE_CODES[data.dtype], b, c, data[0, 0].numel(),
                      _ptr(intensity), _ptr(total), _ptr(flags), _ptr(ws), ws_bytes, _stream(data))
-    _count(2)
     return total, flags
 
 
@@ -1150,7 +1102,6 @@ def spectrum_peak(data: Tensor, intensity: Tensor, flags: Tensor, workspace_byte
     with torch.cuda.device(data.device):
         _native.call("tio_spectrum_peak", _ptr(data), RESOLUTION_DTYPE_CODES[data.dtype], b, c, i, j, k,
                      _ptr(intensity), _ptr(flags), _ptr(peak), _ptr(ws), workspace_bytes, _stream(data))
-    _count(1 + 3 * -(-(b * c) // (workspace_bytes // row_bytes)))
     return peak
 
 
@@ -1194,5 +1145,4 @@ def ghosting(data: Tensor, table: np.ndarray, axis: np.ndarray, active: np.ndarr
         _native.call("tio_ghosting", _ptr(data), RESOLUTION_DTYPE_CODES[data.dtype], b, c, i, j, k, _ptr(table_d),
                      int(table.shape[1]), _ptr(axis_d), _ptr(active_d), sum(1 << a for a in ghosted), _ptr(flags),
                      _stream(data))
-    _count(2 + len(ghosted))
     return data
