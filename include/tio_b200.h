@@ -595,6 +595,27 @@ int tio_spike(void* data, int dtype, int B, int C, int I, int J, int K, const in
 int tio_ghosting(void* data, int dtype, int B, int C, int I, int J, int K, const float* table, int n_max,
                  const int32_t* axis, const uint8_t* active, int axes, uint32_t* flags, void* stream);
 
+/*
+ * Motion (intensity/motion.py:140-561 of the reference: fftn of data.float(); for each of N rigid
+ * transforms, affine_grid + grid_sample (trilinear, zeros padding, align_corners=True), fftn, and
+ * the first-axis k-space rows [s size, (s + 1) size) copied in (the last segment ends at I, with
+ * size = I // (N + 1)); ifftn, .real, .to(dtype), torch.where for per-instance gating).  The FFTs
+ * over J and K cancel, so each line along I becomes
+ *   out = ifft_I(sum_s Hs_s fft_I(x_s)),   Hs_s(f) = (P_s(f) + P_s(-f mod I)) / 2,
+ * with x_0 = float(data), x_s its resampled copies and P_s the indicator of segment s's rows.  Out
+ * of place on contiguous (B, C, I, J, K) batches of any tio_dtype (in and out must not overlap);
+ * I <= 4096, 2 <= segments <= I, B * C <= 65535.
+ *   segments  N + 1
+ *   theta     device fp32 [B][N][12]: segment s's affine_grid matrix (3 x 4, row major) of element b
+ *             at [b][s - 1]; output voxel (i, j, k) samples theta (lin_K[k], lin_J[j], lin_I[i], 1)
+ *             in the (K, J, I) frame, lin_n = linspace(-1, 1, n)
+ *   active    device uint8 [B]: 0 = gated out, the element is copied bit for bit
+ *   flags     device scratch of B * C uint32
+ * A row with a NaN or +-Inf voxel becomes all NaN (the reference's FFT spreads the value).
+ */
+int tio_motion(const void* in, void* out, int dtype, int B, int C, int I, int J, int K, int segments,
+               const float* theta, const uint8_t* active, uint32_t* flags, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -79,6 +79,7 @@ _SIGNATURES = {
     "tio_spectrum_peak": [c_void_p] + [c_int] * 6 + [c_void_p] * 4 + [c_size_t, c_void_p],
     "tio_spike": [c_void_p] + [c_int] * 6 + [c_void_p, c_int] + [c_void_p] * 5 + [c_size_t, c_void_p],
     "tio_ghosting": [c_void_p] + [c_int] * 6 + [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p],
+    "tio_motion": [c_void_p, c_void_p] + [c_int] * 7 + [c_void_p] * 4,
 }
 
 _lib = None

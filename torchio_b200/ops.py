@@ -1146,3 +1146,43 @@ def ghosting(data: Tensor, table: np.ndarray, axis: np.ndarray, active: np.ndarr
                      int(table.shape[1]), _ptr(axis_d), _ptr(active_d), sum(1 << a for a in ghosted), _ptr(flags),
                      _stream(data))
     return data
+
+
+# ---- Motion (intensity/motion.py) ---------------------------------------------------------------
+
+MOTION_MAX_AXIS = 4096  # longest first axis tio_motion's shared-memory FFT holds
+
+
+def motion(data: Tensor, theta: np.ndarray, active: np.ndarray) -> Tensor:
+    """A new (B, C, I, J, K) CUDA tensor of ``data``'s dtype: the reference's `_apply_motion` /
+    `_apply_motion_per_instance` (motion.py:140-561) as one k-space splice along the first axis,
+    ``ifft_I(sum_s Hs_s * fft_I(x_s))``, with the rigidly resampled copies ``x_s`` gathered on the
+    fly.  ``theta``: fp32 (B, N, 12), element b's `_affine_matrices` of segment s at ``[b, s - 1]``;
+    ``active``: (B,) bool, False for an element that is copied unchanged.  Returns ``data`` itself
+    when no element is active.  No host sync."""
+    _require_cuda(data, "motion")
+    if data.dtype not in RESOLUTION_DTYPE_CODES:
+        raise TypeError(f"motion: unsupported dtype {data.dtype}")
+    if data.ndim != 5 or not data.is_contiguous():
+        raise ValueError(f"motion expects a contiguous (B, C, I, J, K) batch, got {tuple(data.shape)}")
+    b, c, i, j, k = (int(s) for s in data.shape)
+    theta = np.ascontiguousarray(theta, dtype=np.float32)
+    active = np.ascontiguousarray(active, dtype=np.uint8)
+    if theta.ndim != 3 or theta.shape[0] != b or theta.shape[1] < 1 or theta.shape[2] != 12 or active.shape != (b,):
+        raise ValueError(f"motion: tables {theta.shape} / {active.shape} for a batch of {b}")
+    if not active.any() or data.numel() == 0:
+        return data
+    segments = int(theta.shape[1]) + 1
+    if i > MOTION_MAX_AXIS:
+        raise NotImplementedError(
+            f"Motion: spatial shape {(i, j, k)} has a first axis longer than {MOTION_MAX_AXIS} points, the longest"
+            f" the line FFT supports")
+    if i // segments == 0:
+        raise ValueError(f"motion: {segments} segments for a first axis of {i} points")
+    theta_d, active_d = upload(data.device, theta, active)
+    out = torch.empty_like(data)
+    flags = torch.empty(b * c, dtype=torch.int32, device=data.device)
+    with torch.cuda.device(data.device):
+        _native.call("tio_motion", _ptr(data), _ptr(out), RESOLUTION_DTYPE_CODES[data.dtype], b, c, i, j, k, segments,
+                     _ptr(theta_d), _ptr(active_d), _ptr(flags), _stream(data))
+    return out

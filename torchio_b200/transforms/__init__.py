@@ -12,11 +12,12 @@ from .orientation import CopyAffine, EnsureShapeMultiple, Reorient, ToReferenceS
 from .resolution import Anisotropy, Resize
 from .spatial import Affine, ElasticDeformation, Resample, Spatial
 from .ghosting import Ghosting
+from .motion import Motion
 from .spike import Spike
 
 __all__ = [
     "Affine", "Anisotropy", "AppliedTransform", "BiasField", "Blur", "Clamp", "Compose", "Contour", "CopyAffine", "Crop", "CropOrPad", "ElasticDeformation", "EnsureShapeMultiple",
-    "Flip", "Gamma", "Ghosting", "HistogramStandardization", "IntensityTransform", "KeepLargestComponent", "LabelsToImage", "Mask", "Noise", "Normalize", "OneHot", "Pad", "RemapLabels",
+    "Flip", "Gamma", "Ghosting", "HistogramStandardization", "IntensityTransform", "KeepLargestComponent", "LabelsToImage", "Mask", "Motion", "Noise", "Normalize", "OneHot", "Pad", "RemapLabels",
     "RemoveLabels", "Reorient", "Resample", "Resize", "RescaleIntensity", "SequentialLabels", "Spatial",
     "SpatialTransform", "Spike", "Standardize", "Swap", "ToReferenceSpace", "Transform", "Transpose", "ZNormalization",
     "apply_inverse_transform", "compute_histogram_landmarks", "execution_device", "get_inverse_transform",
