@@ -616,6 +616,40 @@ int tio_ghosting(void* data, int dtype, int B, int C, int I, int J, int K, const
 int tio_motion(const void* in, void* out, int dtype, int B, int C, int I, int J, int K, int segments,
                const float* theta, const uint8_t* active, uint32_t* flags, void* stream);
 
+/*
+ * PatchAggregator (data/aggregator.py of the reference), one launch per key and batch.
+ *
+ * tio_aggregate_patches adds the first `n` patches of a batch `patches` (B, C, pi, pj, pk) into the
+ * buffer `out` (C, I, J, K), in table order, as the reference's add_batch -> _add_patch does one
+ * patch at a time (aggregator.py:75-100, 143-237):
+ *   mode 0 crop     out[box] = patch[src box]; where boxes overlap, the last one wins
+ *   mode 1 average  out[box] += patch, counts[box] += 1, both in the buffer's dtype
+ *   mode 2 hann     out[box] += patch * window, counts[box] += window, window = (w_i w_j) w_k in fp32
+ *                   (fp64 for an fp64 buffer), rounded once to the buffer's dtype
+ * Integer adds wrap; fp16 / bf16 are computed in fp32 and rounded after each add, as ATen's CPU
+ * ops do.  Voxels no box covers are not written.  No atomics: the result does not depend on
+ * scheduling.
+ *   dtype          tio_dtype code of patches, out and counts; bool moves as TIO_U8 in crop mode;
+ *                  hann needs TIO_F32, TIO_F16, TIO_BF16 or TIO_F64
+ *   counts         (1, I, J, K) device, one channel for every channel of `out` (the reference
+ *                  keeps C equal channels); NULL in crop mode
+ *   boxes          HOST int32 [n][10]: dst lo i, j, k, dst hi i, j, k (exclusive), src lo i, j, k,
+ *                  patch row in 0..B-1; every box non-empty, inside the buffer and inside its patch
+ *                  (checked before any launch); source extent = destination extent
+ *   boxes_device   the same table in device memory (the kernel reads it there)
+ *   window         device fp32 [pi + pj + pk]: torch.hann_window(n + 2, periodic=False)[1:-1] of
+ *                  each patch axis in turn (aggregator.py:239-245); NULL unless mode is hann
+ *
+ * tio_aggregate_finish writes out / counts.clamp(min=1) (aggregator.py:117-120) into `dst`, the
+ * single-channel count broadcast over the C channels of `out` (C, vox).  `dst` has the buffer's
+ * dtype, or fp32 for an integer buffer (true division of integers).
+ */
+int tio_aggregate_patches(const void* patches, void* out, void* counts, int dtype, int mode, int C, int I,
+                          int J, int K, int B, int pi, int pj, int pk, int n, const int32_t* boxes,
+                          const int32_t* boxes_device, const float* window, void* stream);
+int tio_aggregate_finish(const void* out, const void* counts, void* dst, int dtype, int C, int64_t vox,
+                         void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -7,7 +7,7 @@ Drop-in for the reference's spatial + intensity augmentation chain
 `Resize`), histogram standardization (`HistogramStandardization`,
 `ZNormalization`), `Clamp`, `Mask`, `Swap`, `Spike`, `Ghosting`, `Motion`, the orientation and shape
 utilities (`Reorient`, `Transpose`, `EnsureShapeMultiple`, `CopyAffine`, `ToReferenceSpace`) and its patch path (`UniformSampler`, `Queue`,
-`SubjectsLoader`) on tensor-backed `Subject` / `SubjectsBatch` data.  The
+`SubjectsLoader`, `GridSampler`, `PatchAggregator`) on tensor-backed `Subject` / `SubjectsBatch` data.  The
 tensor math runs in hand-written sm_90a (H100) CUDA kernels exposed through the C-ABI
 of ``include/tio_b200.h``; see DESIGN.md and INTEGRATION.md.
 """
@@ -16,7 +16,7 @@ from .data import (AffineMatrix, Image, ImagesBatch, LabelMap, ScalarImage, Stud
                    Subject, SubjectsBatch)
 from .ops import exact_coords_default, set_exact_coords
 from .params import Choice
-from .patches import (GridSampler, ImagesLoader, LabelSampler, PatchLocation, PatchSampler, Queue,
+from .patches import (GridSampler, ImagesLoader, LabelSampler, PatchAggregator, PatchLocation, PatchSampler, Queue,
                       StudiesLoader, SubjectsLoader, UniformSampler, WeightedSampler, collate_images, collate_studies,
                       collate_subjects)
 from .transforms import (Affine, Anisotropy, AppliedTransform, BiasField, Blur, Clamp, Compose, Contour, CopyAffine, Crop, CropOrPad,
@@ -31,7 +31,7 @@ __version__ = "0.1.0"
 __all__ = [
     "Affine", "AffineMatrix", "Anisotropy", "AppliedTransform", "BiasField", "Blur", "Choice", "Clamp", "Compose", "Contour", "CopyAffine", "Crop", "CropOrPad",
     "ElasticDeformation", "EnsureShapeMultiple", "Flip", "Gamma", "Ghosting", "GridSampler", "HistogramStandardization", "Image", "ImagesBatch", "ImagesLoader", "IntensityTransform",
-    "KeepLargestComponent",     "LabelMap", "LabelSampler", "LabelsToImage", "Mask", "Motion", "Noise", "Normalize", "OneHot", "Pad", "PatchLocation", "PatchSampler", "Queue", "RemapLabels", "RemoveLabels",
+    "KeepLargestComponent",     "LabelMap", "LabelSampler", "LabelsToImage", "Mask", "Motion", "Noise", "Normalize", "OneHot", "Pad", "PatchAggregator", "PatchLocation", "PatchSampler", "Queue", "RemapLabels", "RemoveLabels",
     "Reorient", "Resample", "RescaleIntensity", "Resize", "ScalarImage", "SequentialLabels", "Spatial",
     "SpatialTransform", "Spike", "Standardize", "StudiesBatch", "StudiesLoader", "Subject", "SubjectsBatch",
     "SubjectsLoader", "Swap", "ToReferenceSpace", "Transform", "Transpose", "UniformSampler", "WeightedSampler", "ZNormalization", "apply_inverse_transform", "collate_images",

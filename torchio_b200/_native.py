@@ -80,6 +80,8 @@ _SIGNATURES = {
     "tio_spike": [c_void_p] + [c_int] * 6 + [c_void_p, c_int] + [c_void_p] * 5 + [c_size_t, c_void_p],
     "tio_ghosting": [c_void_p] + [c_int] * 6 + [c_void_p, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p],
     "tio_motion": [c_void_p, c_void_p] + [c_int] * 7 + [c_void_p] * 4,
+    "tio_aggregate_patches": [c_void_p] * 3 + [c_int] * 11 + [c_void_p] * 4,
+    "tio_aggregate_finish": [c_void_p] * 3 + [c_int, c_int, c_int64, c_void_p],
 }
 
 _lib = None

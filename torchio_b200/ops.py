@@ -294,6 +294,66 @@ def crop_patches(volume: Tensor, corners, size, out: Tensor | None = None) -> Te
     return dst
 
 
+AGGREGATE_MODES = {"crop": 0, "average": 1, "hann": 2}
+
+
+def aggregate_patches(patches: Tensor, out: Tensor, counts: Tensor | None, boxes: np.ndarray, mode: str,
+                      window: np.ndarray | None = None) -> None:
+    """In place: add the patches of a batch (B, C, pi, pj, pk) into the PatchAggregator buffer ``out``
+    (C, I, J, K) of the same dtype and device, in the order of ``boxes``, as the reference's
+    `_add_crop` / `_add_average` / `_add_hann` do one patch at a time (data/aggregator.py:143-237).
+    ``counts``: the (1, I, J, K) count buffer of "average" and "hann", None for "crop".
+    ``boxes``: int32 (n, 10) rows ``dst lo (3), dst hi (3), src lo (3), patch row``.  ``window``: fp32
+    (pi + pj + pk,), the three 1-D Hann windows of the patch, for "hann" only.  One launch, no host
+    sync."""
+    _require_cuda(patches, "aggregate_patches")
+    _require_cuda(out, "aggregate_patches")
+    if mode not in AGGREGATE_MODES:
+        raise ValueError(f"aggregate_patches: mode {mode!r} not in {tuple(AGGREGATE_MODES)}")
+    if patches.dtype != out.dtype or (counts is not None and counts.dtype != out.dtype):
+        raise TypeError(f"aggregate_patches: patches {patches.dtype} and buffers {out.dtype} differ")
+    dtype = torch.uint8 if out.dtype == torch.bool and mode == "crop" else out.dtype
+    if dtype not in RESOLUTION_DTYPE_CODES:
+        raise TypeError(f"aggregate_patches: unsupported dtype {out.dtype} in {mode} mode")
+    if patches.ndim != 5 or out.ndim != 4 or not out.is_contiguous() or patches.device != out.device:
+        raise ValueError(f"aggregate_patches expects a (B, C, pi, pj, pk) batch and a contiguous (C, I, J, K) buffer"
+                         f" on one device, got {tuple(patches.shape)} and {tuple(out.shape)}")
+    if counts is not None and (tuple(counts.shape) != (1, *out.shape[1:]) or not counts.is_contiguous()
+                               or counts.device != out.device):
+        raise ValueError(f"aggregate_patches: counts {tuple(counts.shape)} for a buffer {tuple(out.shape)}")
+    boxes = np.ascontiguousarray(boxes, dtype=np.int32).reshape(-1, 10)
+    if boxes.shape[0] == 0:
+        return
+    if window is not None:
+        window = np.ascontiguousarray(window, dtype=np.float32)
+    patches = patches.contiguous()
+    b, c, pi, pj, pk = (int(s) for s in patches.shape)
+    boxes_d, window_d = upload(out.device, boxes, window)
+    with torch.cuda.device(out.device):
+        _native.call("tio_aggregate_patches", _ptr(patches), _ptr(out), _ptr(counts), RESOLUTION_DTYPE_CODES[dtype],
+                     AGGREGATE_MODES[mode], *(int(s) for s in out.shape), b, pi, pj, pk, int(boxes.shape[0]),
+                     boxes.ctypes.data, _ptr(boxes_d), _ptr(window_d), _stream(out))
+
+
+def aggregate_finish(out: Tensor, counts: Tensor) -> Tensor:
+    """A new tensor ``out / counts.clamp(min=1)`` (data/aggregator.py:117-120) for a PatchAggregator
+    buffer (C, I, J, K) and its (1, I, J, K) count: the buffer's dtype, fp32 for integers.  One launch."""
+    _require_cuda(out, "aggregate_finish")
+    if out.dtype not in RESOLUTION_DTYPE_CODES or counts.dtype != out.dtype:
+        raise TypeError(f"aggregate_finish: unsupported dtypes {out.dtype} / {counts.dtype}")
+    if (out.ndim != 4 or tuple(counts.shape) != (1, *out.shape[1:]) or not out.is_contiguous()
+            or not counts.is_contiguous() or counts.device != out.device):
+        raise ValueError(f"aggregate_finish: buffer {tuple(out.shape)} and counts {tuple(counts.shape)}")
+    floating = out.dtype.is_floating_point
+    dst = torch.empty(out.shape, dtype=out.dtype if floating else torch.float32, device=out.device)
+    if out.numel() == 0:
+        return dst
+    with torch.cuda.device(out.device):
+        _native.call("tio_aggregate_finish", _ptr(out), _ptr(counts), _ptr(dst), RESOLUTION_DTYPE_CODES[out.dtype],
+                     int(out.shape[0]), out[0].numel(), _stream(out))
+    return dst
+
+
 PAD_MODES = {"constant": 0, "replicate": 1, "reflect": 2, "circular": 3}
 
 

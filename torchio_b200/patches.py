@@ -188,6 +188,170 @@ class GridSampler(PatchSampler, Dataset):
                 for i in per_axis[0] for j in per_axis[1] for k in per_axis[2]]
 
 
+# ---------------------------------------------------------------------------------------
+# PatchAggregator: stitch inference patches back into a volume (data/aggregator.py:12-245)
+#
+# The reference moves every batch to the host and adds its patches one at a time.  Here the
+# buffers stay on the device and each `add_batch` is one `tio_aggregate_patches` launch per key:
+# the boxes are resolved on the host from the locations alone (Python slice rules, as the
+# reference's slicing), checked against the patch shape for the whole batch, and uploaded as one
+# table.  Counts are kept as one channel: their update does not depend on the channel.
+# ---------------------------------------------------------------------------------------
+
+_AGGREGATOR_MODES = ("crop", "average", "hann")
+_ATEN_NAMES = {torch.uint8: "Byte", torch.int8: "Char", torch.int16: "Short", torch.int32: "Int",
+               torch.int64: "Long", torch.bool: "Bool"}
+
+
+def _resolved(start: int, stop: int, n: int) -> tuple[int, int]:
+    """``t[start:stop]`` of an axis of ``n`` points as (first index, length)."""
+    first, last, _ = slice(start, stop).indices(n)
+    return first, max(0, last - first)
+
+
+class PatchAggregator:
+    """Reassemble patches into a full volume (data/aggregator.py:12-245).
+
+    Same constructor, attributes, modes ("crop", "average", "hann") and results as the reference,
+    which it reproduces bit for bit.  The buffers live on the device of the first batch added (on
+    `execution_device()` when that batch is on the host); `get_output` returns a tensor on the device
+    of that first batch.  Differences: a batch is checked as a whole before anything is added, a
+    box that only broadcasting would fit and a batch whose dtype differs from the buffer's raise
+    `NotImplementedError`, and the counts are one channel instead of C equal ones."""
+
+    def __init__(self, spatial_shape, overlap_mode: str = "crop", patch_overlap=0, output_shape=None) -> None:
+        if overlap_mode not in _AGGREGATOR_MODES:
+            raise ValueError(f"overlap_mode must be one of {_AGGREGATOR_MODES}, got {overlap_mode!r}")
+        self.input_spatial_shape = spatial_shape
+        self.overlap_mode = overlap_mode
+        if isinstance(patch_overlap, int):
+            patch_overlap = (patch_overlap, patch_overlap, patch_overlap)
+        self.patch_overlap = patch_overlap
+        if output_shape is not None:
+            self.spatial_shape = output_shape
+            self._scale = tuple(output_shape[a] / spatial_shape[a] for a in range(3))
+        else:
+            self.spatial_shape = spatial_shape
+            self._scale = (1.0, 1.0, 1.0)
+        self._outputs: dict[str, torch.Tensor] = {}
+        self._counts: dict[str, torch.Tensor] = {}
+        self._device: torch.device | None = None
+        self._host_caller = False
+
+    def _box(self, location: PatchLocation, patch_shape) -> tuple[tuple[int, int, int], tuple[int, int, int],
+                                                                  tuple[int, int, int], tuple[int, int, int]]:
+        """Where the reference writes a patch of spatial shape ``patch_shape`` added at ``location``:
+        (first destination voxel, destination extent, first source voxel, source extent) per axis,
+        the location scaled first when there is an ``output_shape`` (aggregator.py:93-96, 153-237)."""
+        if self._scale != (1.0, 1.0, 1.0):
+            location = location.scaled(self._scale)
+        ini, fin = list(location.index_ini), list(location.index_fin)
+        crop_ini, crop_fin = [0, 0, 0], list(patch_shape)
+        if self.overlap_mode == "crop":
+            crop_fin = list(location.size)
+            for a in range(3):
+                half = round(self.patch_overlap[a] * self._scale[a]) // 2
+                if ini[a] > 0:
+                    ini[a] += half
+                    crop_ini[a] += half
+                if fin[a] < self.spatial_shape[a]:
+                    fin[a] -= half
+                    crop_fin[a] -= half
+        dst = [_resolved(ini[a], fin[a], self.spatial_shape[a]) for a in range(3)]
+        src = [_resolved(crop_ini[a], crop_fin[a], patch_shape[a]) for a in range(3)]
+        return (tuple(d[0] for d in dst), tuple(d[1] for d in dst), tuple(s[0] for s in src),
+                tuple(s[1] for s in src))
+
+    def _device_for(self, tensor: torch.Tensor) -> torch.device:
+        if self._device is None:
+            self._host_caller = not tensor.is_cuda
+            if tensor.is_cuda:
+                self._device = tensor.device
+            else:
+                from .transforms.base import execution_device
+
+                self._device = execution_device()
+        return self._device
+
+    def _check_dtype(self, key: str, tensor: torch.Tensor) -> None:
+        dtype, mode = tensor.dtype, self.overlap_mode
+        if mode == "hann" and not dtype.is_floating_point:
+            raise RuntimeError(f"result type Float can't be cast to the desired output type {_ATEN_NAMES[dtype]}")
+        if mode == "average" and dtype == torch.bool:
+            raise RuntimeError("result type Long can't be cast to the desired output type Bool")
+        if key in self._outputs and self._outputs[key].dtype != dtype:
+            raise NotImplementedError(
+                f"PatchAggregator: a batch of {dtype} for key {key!r}, whose buffer is {self._outputs[key].dtype};"
+                f" the reference casts it by type promotion, cast it before add_batch")
+
+    def _table(self, key: str, tensor: torch.Tensor, locations) -> np.ndarray:
+        """The batch's box table (n, 10), every box checked against its patch first."""
+        if tensor.ndim != 5:
+            raise ValueError(f"PatchAggregator.add_batch expects (B, C, I, J, K) tensors, got {tuple(tensor.shape)}"
+                             f" for key {key!r}")
+        if len(locations) > tensor.shape[0]:
+            raise IndexError(f"index {tensor.shape[0]} is out of bounds for dimension 0 with size {tensor.shape[0]}")
+        self._check_dtype(key, tensor)
+        channels = self._outputs[key].shape[0] if key in self._outputs else tensor.shape[1]
+        patch_shape = tuple(tensor.shape[2:])
+        rows = []
+        for row, location in enumerate(locations):
+            dst_lo, dst_len, src_lo, src_len = self._box(location, patch_shape)
+            target, value = (channels, *dst_len), (tensor.shape[1], *src_len)
+            if target != value:
+                bad = [d for d in range(4) if value[d] not in (target[d], 1)]
+                if bad:
+                    raise RuntimeError(
+                        f"The size of tensor a ({target[bad[0]]}) must match the size of tensor b ({value[bad[0]]})"
+                        f" at non-singleton dimension {bad[0]}: patch {row} of key {key!r} has shape {list(value)},"
+                        f" its box {list(target)}")
+                raise NotImplementedError(
+                    f"PatchAggregator: patch {row} of key {key!r} has shape {list(value)} and fits its box"
+                    f" {list(target)} only by broadcasting, which the aggregator does not do")
+            if min(dst_len) > 0 and channels > 0:
+                rows.append([*dst_lo, *(dst_lo[a] + dst_len[a] for a in range(3)), *src_lo, row])
+        return np.asarray(rows, dtype=np.int32).reshape(-1, 10)
+
+    def add_batch(self, batch, locations) -> None:
+        """Add a batch of model outputs, a (B, C, I, J, K) tensor or a dict of them keyed by name, whose
+        first ``len(locations)`` patches lie at ``locations`` (aggregator.py:75-100).  The whole batch
+        is checked before any of it is added; device batches take one launch per key, no host sync."""
+        tensors = {"__default__": batch} if isinstance(batch, torch.Tensor) else dict(batch)
+        if not tensors or not len(locations):
+            return
+        tables = {key: self._table(key, tensor, locations) for key, tensor in tensors.items()}
+        device = self._device_for(next(iter(tensors.values())))
+        staged = []
+        for key, tensor in tensors.items():
+            tensor = tensor if tensor.device == device else tensor.to(device)
+            ops._require_cuda(tensor, "aggregate_patches")
+            staged.append((key, tensor, tables[key]))
+        for key, tensor, table in staged:
+            if key not in self._outputs:
+                self._outputs[key] = torch.zeros((tensor.shape[1], *self.spatial_shape), dtype=tensor.dtype,
+                                                 device=device)
+                if self.overlap_mode != "crop":
+                    self._counts[key] = torch.zeros((1, *self.spatial_shape), dtype=tensor.dtype, device=device)
+            window = None
+            if self.overlap_mode == "hann":
+                window = torch.cat([torch.hann_window(n + 2, periodic=False)[1:-1] for n in tensor.shape[2:]])
+            ops.aggregate_patches(tensor, self._outputs[key], self._counts.get(key), table, self.overlap_mode,
+                                  window)
+
+    def get_output(self, key: str | None = None) -> torch.Tensor:
+        """The aggregated (C, I, J, K) volume (aggregator.py:102-123): "crop" returns the buffer itself
+        (a host copy for a caller whose first batch was on the host), "average" and "hann" a new
+        tensor ``out / counts.clamp(min=1)``, fp32 for integer buffers."""
+        resolve_key = key if key is not None else "__default__"
+        if resolve_key not in self._outputs:
+            available = [k for k in self._outputs if k != "__default__"]
+            raise KeyError(f"No output for key {key!r}. Available: {available}")
+        output = self._outputs[resolve_key]
+        if self.overlap_mode != "crop":
+            output = ops.aggregate_finish(output, self._counts[resolve_key])
+        return output.cpu() if self._host_caller else output
+
+
 def _mask_borders(prob: torch.Tensor, spatial_shape, patch_size) -> torch.Tensor:
     """Zero probability where a patch centre cannot be placed (data/sampler.py:340-360)."""
     prob = prob.clone()
