@@ -1,6 +1,6 @@
-"""The boundary is executable: the header, the product's own ctypes binding and the stub printed in
-INTEGRATION.md (what a TorchIO maintainer would paste) must agree argument for argument, and the
-stub — run verbatim — must reproduce `ops.resample` on a golden case."""
+"""The boundary is executable: the product binds every function from include/tio_b200.h itself, the
+stub printed in INTEGRATION.md (what a TorchIO maintainer would paste) must agree with the header
+argument for argument, and the stub — run verbatim — must reproduce `ops.resample` on a golden case."""
 
 import ctypes
 import re
@@ -13,22 +13,11 @@ import torch
 from torchio_b200 import _native
 
 ROOT = Path(__file__).resolve().parent.parent
-C2CTYPES = {"float": ctypes.c_float, "int": ctypes.c_int, "int64_t": ctypes.c_int64, "uint64_t": ctypes.c_uint64, "size_t": ctypes.c_size_t}
 
 
 def header_prototypes():
-    """name -> list of ctypes argument types, parsed from include/tio_b200.h."""
-    text = re.sub(r"/\*.*?\*/", "", (ROOT / "include" / "tio_b200.h").read_text(), flags=re.S)
-    out = {}
-    for m in re.finditer(r"(?:const\s+char\s*\*|size_t|int)\s+(tio_\w+)\s*\(([^)]*)\)\s*;", text):
-        name, args = m.group(1), m.group(2).strip()
-        types = []
-        if args not in ("", "void"):
-            for a in args.split(","):
-                ctype = re.sub(r"\s+\w+$", "", a.strip())
-                types.append(ctypes.c_void_p if "*" in ctype else C2CTYPES[ctype])
-        out[name] = types
-    return out
+    """name -> list of ctypes argument types, as the product parses them from include/tio_b200.h."""
+    return {name: argtypes for name, (_, argtypes) in _native.prototypes().items()}
 
 
 def integration_blocks():
@@ -47,11 +36,41 @@ class _Recorder:
         return self.fns.setdefault(name, type("F", (), {})())
 
 
-def test_product_binding_matches_the_header_argument_for_argument():
-    protos = header_prototypes()
-    assert set(protos) - {"tio_last_error"} == set(_native._SIGNATURES)
-    for name, argtypes in _native._SIGNATURES.items():
-        assert argtypes == protos[name], name
+def test_every_declared_function_is_bound_with_the_header_types():
+    protos = _native.prototypes()
+    text = re.sub(r"/\*.*?\*/", "", (ROOT / "include" / "tio_b200.h").read_text(), flags=re.S)
+    assert sorted(protos) == sorted(re.findall(r"\b(tio_\w+)\s*\(", text))
+    lib = _native.lib()
+    for name, (restype, argtypes) in protos.items():
+        fn = getattr(lib, name)
+        assert fn.restype is restype and list(fn.argtypes) == argtypes, name
+    P, I32, I64, U64, SZ, F32 = (ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_uint64, ctypes.c_size_t,
+                                 ctypes.c_float)
+    assert protos["tio_rescale"] == (I32, [P, P, I32, I64, F32, F32, P, P, P, P, P, I32, P])
+    assert protos["tio_label_argmax"] == (I32, [P, I32, I32, I64, P, F32, P, I32, P])
+    assert protos["tio_randn_mt19937"] == (I32, [U64, U64, U64, P, P, P, SZ, P])
+    assert protos["tio_quantiles"] == (I32, [P, P, I64, P, I32, P, P, P, P, SZ, P])
+    assert protos["tio_quantiles_workspace_bytes"] == (SZ, [])
+    assert protos["tio_launch_count"] == (U64, [])
+    assert protos["tio_last_error"] == (ctypes.c_char_p, [])
+
+
+@pytest.mark.parametrize("declaration,message", [
+    ("double tio_extra(void);", "does not map"),
+    ("int tio_extra(unsigned n, void* stream);", "does not map"),
+    ("int tio_extra(void (*done)(int), void* stream);", "prototypes could be parsed"),
+], ids=["return-type", "argument-type", "skipped-declaration"])
+def test_a_header_the_binding_cannot_read_whole_is_refused(tmp_path, monkeypatch, declaration, message):
+    header = tmp_path / "tio_b200.h"
+    text = _native.HEADER_PATH.read_text()
+    header.write_text(text.replace("#ifdef __cplusplus\n}", f"{declaration}\n#ifdef __cplusplus\n}}"))
+    monkeypatch.setattr(_native, "HEADER_PATH", header)
+    _native.prototypes.cache_clear()
+    try:
+        with pytest.raises(RuntimeError, match=message):
+            _native.prototypes()
+    finally:
+        _native.prototypes.cache_clear()
 
 
 def test_integration_md_argtypes_match_the_header():

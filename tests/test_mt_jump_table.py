@@ -83,3 +83,13 @@ def test_jump_polynomial_matches_cpu_generator(table, level):
     want = _untemper(bg.random_raw(624).astype(np.uint32))
     assert np.array_equal(out[1:], want[1:])
     assert out[0] >> 31 == want[0] >> 31
+
+
+def test_device_table_of_cuda_without_an_index_is_the_current_devices(monkeypatch):
+    """`randn_mt19937(..., "cuda")` runs on the current device, so it must read that device's table,
+    whichever device the table was first copied to."""
+    monkeypatch.setattr(ops, "_mt_device_tables", {0: "table on cuda:0", 1: "table on cuda:1"})
+    for current in (0, 1):
+        monkeypatch.setattr(torch.cuda, "current_device", lambda current=current: current)
+        assert ops._mt_table(torch.device("cuda")) == f"table on cuda:{current}"
+        assert ops._mt_table(torch.device("cuda", 1 - current)) == f"table on cuda:{1 - current}"

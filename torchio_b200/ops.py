@@ -22,6 +22,9 @@ DTYPE_CODES = {
     torch.float32: 0, torch.uint8: 1, torch.int8: 2,
     torch.int16: 3, torch.int32: 4, torch.int64: 5,
 }
+# every label dtype, and fp16 / bf16 / fp64 images, which the kernels compute in fp32 and cast back
+# as the reference's data.float() ... .to(dtype) do (tio_dtype TIO_F16 / TIO_BF16 / TIO_F64)
+IMAGE_DTYPE_CODES = {**DTYPE_CODES, torch.float16: 6, torch.bfloat16: 7, torch.float64: 8}
 NEAREST, LINEAR, LABEL_PV = 0, 1, 2
 FLAG_PASSTHROUGH, FLAG_ELASTIC = 1, 2
 
@@ -31,15 +34,20 @@ def launches() -> int:
     return _native.lib().tio_launch_count()
 
 
-def _stream(t: Tensor) -> int:
-    return torch.cuda.current_stream(t.device).cuda_stream
+def _launch(name: str, device, *args) -> None:
+    """Call the stream-taking entry point ``name`` with ``args`` and the current stream of
+    ``device``, with ``device`` current: CUDA refuses a launch into another device's stream."""
+    with torch.cuda.device(device):
+        _native.call(name, *args, torch.cuda.current_stream(device).cuda_stream)
 
 
 def _ptr(t: Tensor | None):
     return None if t is None else t.data_ptr()
 
 
-def _require_cuda(t: Tensor, name: str) -> None:
+def _check(t: Tensor, name: str, *, dtypes=None, ndim: int | None = 5) -> None:
+    """Refuse ``t`` as an input of ops.``name`` unless it is a CUDA tensor that does not require
+    grad, of a dtype in ``dtypes`` (None: any) with ``ndim`` dimensions (None: any)."""
     if not t.is_cuda:
         raise RuntimeError(
             f"torchio_b200.ops.{name}: expected a CUDA tensor (got {t.device});"
@@ -49,6 +57,21 @@ def _require_cuda(t: Tensor, name: str) -> None:
         raise NotImplementedError(
             f"torchio_b200.ops.{name}: kernels are forward-only; detach() the input"
         )
+    if dtypes is not None and t.dtype not in dtypes:
+        raise TypeError(f"{name}: unsupported dtype {t.dtype}")
+    if ndim is not None and t.ndim != ndim:
+        raise ValueError(f"{name} expects a {ndim}-D tensor, got {tuple(t.shape)}")
+
+
+def _batch(t: Tensor, name: str, *, dtypes=None, ndim: int | None = 5, in_place: bool = False) -> Tensor:
+    """``t`` checked by `_check` and returned contiguous: a non-contiguous ``t`` is copied, or
+    refused when ``in_place`` (the op uses ``t`` itself)."""
+    _check(t, name, dtypes=dtypes, ndim=ndim)
+    if not in_place:
+        return t.contiguous()
+    if not t.is_contiguous():
+        raise ValueError(f"{name} expects a contiguous tensor, got strides {t.stride()}")
+    return t
 
 
 class _StagingRing:
@@ -132,8 +155,7 @@ def upload(device: torch.device, *arrays):
     if slot is not None:
         # SM copy kernel instead of cudaMemcpyAsync: see tio_upload in include/tio_b200.h
         dev = torch.empty(offset, dtype=torch.uint8, device=device)
-        _native.call("tio_upload", stage.data_ptr(), dev.data_ptr(), offset,
-                     torch.cuda.current_stream(dev.device).cuda_stream)
+        _launch("tio_upload", dev.device, stage.data_ptr(), dev.data_ptr(), offset)
         _ring.release(slot, torch.device(device))
     else:
         dev = stage.to(device, non_blocking=True)
@@ -181,10 +203,7 @@ def resample(
     from the reference by its own coordinate noise (<= ~2e-5 voxel); label maps, padding and
     fill decisions are exact either way.
     """
-    _require_cuda(src, "resample")
-    if src.dtype not in DTYPE_CODES:
-        raise TypeError(f"resample: unsupported dtype {src.dtype}")
-    src = src.contiguous()
+    src = _batch(src, "resample", dtypes=DTYPE_CODES)
     b, c, i, j, k = src.shape
     oi, oj, ok = (i, j, k) if out_shape is None else out_shape
     dst = torch.empty((b, c, oi, oj, ok), dtype=src.dtype, device=src.device)
@@ -199,65 +218,55 @@ def resample(
     if box_hint >= 0 and tiled:
         ws_bytes = _native.lib().tio_resample_workspace_bytes(b, oi, oj, ok)
         workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=src.device)
-    with torch.cuda.device(src.device):
-        _native.call(
-            "tio_resample", _ptr(src), _ptr(dst), DTYPE_CODES[src.dtype],
-            b, c, i, j, k, oi, oj, ok, _ptr(mat), _ptr(cp), _ptr(flags), ni, nj, nk,
-            sp_in.ctypes.data, sp_out.ctypes.data, int(bool(affine_first)),
-            int(mode) | (EXACT_COORDS if (_exact_default if exact_coords is None else exact_coords) else 0),
-            _ptr(fill), int(box_hint), _ptr(workspace), ws_bytes, _stream(src),
-        )
+    _launch(
+        "tio_resample", src.device, _ptr(src), _ptr(dst), DTYPE_CODES[src.dtype],
+        b, c, i, j, k, oi, oj, ok, _ptr(mat), _ptr(cp), _ptr(flags), ni, nj, nk,
+        sp_in.ctypes.data, sp_out.ctypes.data, int(bool(affine_first)),
+        int(mode) | (EXACT_COORDS if (_exact_default if exact_coords is None else exact_coords) else 0),
+        _ptr(fill), int(box_hint), _ptr(workspace), ws_bytes,
+    )
     return dst
 
 
-def _label_table(labels: Tensor, dtype: torch.dtype) -> Tensor:
-    return labels.to(torch.float32 if dtype == torch.float32 else torch.int64).contiguous()
+def _label_table(labels: Tensor, dtype: torch.dtype, device: torch.device) -> Tensor:
+    return labels.to(device=device, dtype=torch.float32 if dtype == torch.float32 else torch.int64).contiguous()
 
 
 def onehot(src: Tensor, labels: Tensor) -> Tensor:
     """(B,1,I,J,K) label batch -> (B,n,I,J,K) fp32 one-hot channels, ``labels`` = the distinct
     values in ascending order (spatial/spatial.py:1362-1365)."""
-    _require_cuda(src, "onehot")
-    if src.dtype not in DTYPE_CODES:
-        raise TypeError(f"onehot: unsupported dtype {src.dtype}")
-    src = src.contiguous()
+    src = _batch(src, "onehot", dtypes=DTYPE_CODES, ndim=None)
     b, n = src.shape[0], int(labels.numel())
     vox = src[0].numel()
-    table = _label_table(labels, src.dtype)
+    table = _label_table(labels, src.dtype, src.device)
     dst = torch.empty((b, n, *src.shape[2:]), dtype=torch.float32, device=src.device)
-    with torch.cuda.device(src.device):
-        _native.call("tio_onehot", _ptr(src), DTYPE_CODES[src.dtype], b, vox, _ptr(table), n, _ptr(dst),
-                     _stream(src))
+    _launch("tio_onehot", src.device, _ptr(src), DTYPE_CODES[src.dtype], b, vox, _ptr(table), n, _ptr(dst))
     return dst
 
 
 def label_argmax(sampled: Tensor, labels: Tensor, pad_label: float, dtype: torch.dtype) -> Tensor:
     """(B,n,I,J,K) sampled one-hot channels -> (B,1,I,J,K) labels of ``dtype``: first maximum over
     the channels, ``pad_label`` where their sum is not > 0.5 (spatial/spatial.py:1378-1389)."""
-    _require_cuda(sampled, "label_argmax")
+    sampled = _batch(sampled, "label_argmax", ndim=None)
     if dtype not in DTYPE_CODES:
         raise TypeError(f"label_argmax: unsupported dtype {dtype}")
-    sampled = sampled.contiguous()
     b, n = sampled.shape[:2]
     vox = sampled[0, 0].numel()
-    table = _label_table(labels, dtype)
+    table = _label_table(labels, dtype, sampled.device)
     dst = torch.empty((b, 1, *sampled.shape[2:]), dtype=dtype, device=sampled.device)
-    with torch.cuda.device(sampled.device):
-        _native.call("tio_label_argmax", _ptr(sampled), b, n, vox, _ptr(table), float(pad_label), _ptr(dst),
-                     DTYPE_CODES[dtype], _stream(sampled))
+    _launch("tio_label_argmax", sampled.device, _ptr(sampled), b, n, vox, _ptr(table), float(pad_label), _ptr(dst),
+            DTYPE_CODES[dtype])
     return dst
 
 
 def min_sample0(src: Tensor) -> Tensor:
     """Per-channel min of batch element 0, on device, no sync
     (spatial/spatial.py:2054-2060,2094-2095)."""
-    _require_cuda(src, "min_sample0")
-    src = src.contiguous()
+    src = _batch(src, "min_sample0", ndim=None)
     c = src.shape[1]
     n = src[0, 0].numel()
     fill = torch.empty(c, dtype=torch.float32, device=src.device)
-    with torch.cuda.device(src.device):
-        _native.call("tio_min_sample0", _ptr(src), c, n, _ptr(fill), _stream(src))
+    _launch("tio_min_sample0", src.device, _ptr(src), c, n, _ptr(fill))
     return fill
 
 
@@ -266,10 +275,7 @@ def crop_patches(volume: Tensor, corners, size, out: Tensor | None = None) -> Te
     (C,I,J,K) into a dense (n,C,*size) block in a single launch
     (data/sampler.py:54-67 + loader.py:15-24).  ``out``: a contiguous (n,C,*size) block to
     write into (e.g. consecutive slots of a patch ring) instead of a fresh tensor."""
-    _require_cuda(volume, "crop_patches")
-    if volume.ndim != 4:
-        raise ValueError(f"crop_patches expects a (C, I, J, K) volume, got {tuple(volume.shape)}")
-    volume = volume.contiguous()
+    volume = _batch(volume, "crop_patches", ndim=4)
     corners = np.ascontiguousarray(np.asarray(corners, dtype=np.int32).reshape(-1, 3))
     n = corners.shape[0]
     c, i, j, k = (int(v) for v in volume.shape)
@@ -286,11 +292,8 @@ def crop_patches(volume: Tensor, corners, size, out: Tensor | None = None) -> Te
         if (tuple(dst.shape) != (n, c, pi, pj, pk) or dst.dtype != volume.dtype or dst.device != volume.device
                 or not dst.is_contiguous()):
             raise ValueError("crop_patches: `out` must be a contiguous (n, C, *size) block of the volume's dtype/device")
-    with torch.cuda.device(volume.device):
-        _native.call(
-            "tio_crop_patches", _ptr(volume), _ptr(dst), volume.element_size(), c, i, j, k, n,
-            _ptr(corners_d), pi, pj, pk, _stream(volume),
-        )
+    _launch("tio_crop_patches", volume.device, _ptr(volume), _ptr(dst), volume.element_size(), c, i, j, k, n,
+            _ptr(corners_d), pi, pj, pk)
     return dst
 
 
@@ -306,18 +309,17 @@ def aggregate_patches(patches: Tensor, out: Tensor, counts: Tensor | None, boxes
     ``boxes``: int32 (n, 10) rows ``dst lo (3), dst hi (3), src lo (3), patch row``.  ``window``: fp32
     (pi + pj + pk,), the three 1-D Hann windows of the patch, for "hann" only.  One launch, no host
     sync."""
-    _require_cuda(patches, "aggregate_patches")
-    _require_cuda(out, "aggregate_patches")
+    _check(patches, "aggregate_patches")
+    out = _batch(out, "aggregate_patches", ndim=4, in_place=True)
     if mode not in AGGREGATE_MODES:
         raise ValueError(f"aggregate_patches: mode {mode!r} not in {tuple(AGGREGATE_MODES)}")
     if patches.dtype != out.dtype or (counts is not None and counts.dtype != out.dtype):
         raise TypeError(f"aggregate_patches: patches {patches.dtype} and buffers {out.dtype} differ")
     dtype = torch.uint8 if out.dtype == torch.bool and mode == "crop" else out.dtype
-    if dtype not in RESOLUTION_DTYPE_CODES:
+    if dtype not in IMAGE_DTYPE_CODES:
         raise TypeError(f"aggregate_patches: unsupported dtype {out.dtype} in {mode} mode")
-    if patches.ndim != 5 or out.ndim != 4 or not out.is_contiguous() or patches.device != out.device:
-        raise ValueError(f"aggregate_patches expects a (B, C, pi, pj, pk) batch and a contiguous (C, I, J, K) buffer"
-                         f" on one device, got {tuple(patches.shape)} and {tuple(out.shape)}")
+    if patches.device != out.device:
+        raise ValueError(f"aggregate_patches: patches on {patches.device}, buffer on {out.device}")
     if counts is not None and (tuple(counts.shape) != (1, *out.shape[1:]) or not counts.is_contiguous()
                                or counts.device != out.device):
         raise ValueError(f"aggregate_patches: counts {tuple(counts.shape)} for a buffer {tuple(out.shape)}")
@@ -329,28 +331,25 @@ def aggregate_patches(patches: Tensor, out: Tensor, counts: Tensor | None, boxes
     patches = patches.contiguous()
     b, c, pi, pj, pk = (int(s) for s in patches.shape)
     boxes_d, window_d = upload(out.device, boxes, window)
-    with torch.cuda.device(out.device):
-        _native.call("tio_aggregate_patches", _ptr(patches), _ptr(out), _ptr(counts), RESOLUTION_DTYPE_CODES[dtype],
-                     AGGREGATE_MODES[mode], *(int(s) for s in out.shape), b, pi, pj, pk, int(boxes.shape[0]),
-                     boxes.ctypes.data, _ptr(boxes_d), _ptr(window_d), _stream(out))
+    _launch("tio_aggregate_patches", out.device, _ptr(patches), _ptr(out), _ptr(counts), IMAGE_DTYPE_CODES[dtype],
+            AGGREGATE_MODES[mode], *(int(s) for s in out.shape), b, pi, pj, pk, int(boxes.shape[0]),
+            boxes.ctypes.data, _ptr(boxes_d), _ptr(window_d))
 
 
 def aggregate_finish(out: Tensor, counts: Tensor) -> Tensor:
     """A new tensor ``out / counts.clamp(min=1)`` (data/aggregator.py:117-120) for a PatchAggregator
     buffer (C, I, J, K) and its (1, I, J, K) count: the buffer's dtype, fp32 for integers.  One launch."""
-    _require_cuda(out, "aggregate_finish")
-    if out.dtype not in RESOLUTION_DTYPE_CODES or counts.dtype != out.dtype:
+    out = _batch(out, "aggregate_finish", dtypes=IMAGE_DTYPE_CODES, ndim=4, in_place=True)
+    if counts.dtype != out.dtype:
         raise TypeError(f"aggregate_finish: unsupported dtypes {out.dtype} / {counts.dtype}")
-    if (out.ndim != 4 or tuple(counts.shape) != (1, *out.shape[1:]) or not out.is_contiguous()
-            or not counts.is_contiguous() or counts.device != out.device):
+    if tuple(counts.shape) != (1, *out.shape[1:]) or not counts.is_contiguous() or counts.device != out.device:
         raise ValueError(f"aggregate_finish: buffer {tuple(out.shape)} and counts {tuple(counts.shape)}")
     floating = out.dtype.is_floating_point
     dst = torch.empty(out.shape, dtype=out.dtype if floating else torch.float32, device=out.device)
     if out.numel() == 0:
         return dst
-    with torch.cuda.device(out.device):
-        _native.call("tio_aggregate_finish", _ptr(out), _ptr(counts), _ptr(dst), RESOLUTION_DTYPE_CODES[out.dtype],
-                     int(out.shape[0]), out[0].numel(), _stream(out))
+    _launch("tio_aggregate_finish", out.device, _ptr(out), _ptr(counts), _ptr(dst), IMAGE_DTYPE_CODES[out.dtype],
+            int(out.shape[0]), out[0].numel())
     return dst
 
 
@@ -362,10 +361,7 @@ def remap(src: Tensor, out_shape, offsets, *, mode: str = "constant", fill=0, fl
     """Flip / Crop / Pad in one pass: ``out[..., o] = src[..., o - offset]`` per spatial
     axis with F.pad's out-of-range rules, then per-element axis reversal (``flip``: (B,)
     uint8 cuda, bit 0 I, 1 J, 2 K).  flip.py:233-263, crop.py:84-101, _padding.py:73-104."""
-    _require_cuda(src, "remap")
-    if src.ndim != 5:
-        raise ValueError(f"remap expects (B, C, I, J, K), got {tuple(src.shape)}")
-    src = src.contiguous()
+    src = _batch(src, "remap")
     b, c, i, j, k = (int(v) for v in src.shape)
     oi, oj, ok = (int(v) for v in out_shape)
     if out is None:
@@ -376,12 +372,8 @@ def remap(src: Tensor, out_shape, offsets, *, mode: str = "constant", fill=0, fl
                 or not dst.is_contiguous()):
             raise ValueError("remap: `out` must be a contiguous (B, C, *out_shape) block of the source's dtype/device")
     fill_host = torch.tensor([fill]).to(src.dtype)  # F.pad casts the value to the tensor's dtype
-    with torch.cuda.device(src.device):
-        _native.call(
-            "tio_remap", _ptr(src), _ptr(dst), src.element_size(), b, c, i, j, k, oi, oj, ok,
-            int(offsets[0]), int(offsets[1]), int(offsets[2]), PAD_MODES[mode],
-            fill_host.data_ptr(), _ptr(flip), _stream(src),
-        )
+    _launch("tio_remap", src.device, _ptr(src), _ptr(dst), src.element_size(), b, c, i, j, k, oi, oj, ok,
+            int(offsets[0]), int(offsets[1]), int(offsets[2]), PAD_MODES[mode], fill_host.data_ptr(), _ptr(flip))
     return dst
 
 
@@ -391,9 +383,7 @@ def permute(src: Tensor, perm, flip_bits: int = 0) -> Tensor:
     input axis, applied before the transpose).  The identity permutation flips through `remap`
     with the same bits for every element, or returns ``src`` itself when nothing flips, as the
     reference does.  reorient.py:63-91, transpose.py:36-50."""
-    _require_cuda(src, "permute")
-    if src.ndim != 5:
-        raise ValueError(f"permute expects (B, C, I, J, K), got {tuple(src.shape)}")
+    _check(src, "permute")
     perm = tuple(int(p) for p in perm)
     if sorted(perm) != [0, 1, 2]:
         raise ValueError(f"permute: {perm} is not a permutation of (0, 1, 2)")
@@ -407,25 +397,19 @@ def permute(src: Tensor, perm, flip_bits: int = 0) -> Tensor:
     b, c, i, j, k = (int(v) for v in src.shape)
     n = (i, j, k)
     dst = torch.empty((b, c, *(n[p] for p in perm)), dtype=src.dtype, device=src.device)
-    with torch.cuda.device(src.device):
-        _native.call("tio_permute", _ptr(src), _ptr(dst), src.element_size(), b, c, i, j, k, *perm, flip_bits,
-                     _stream(src))
+    _launch("tio_permute", src.device, _ptr(src), _ptr(dst), src.element_size(), b, c, i, j, k, *perm, flip_bits)
     return dst
 
 
 def blur(src: Tensor, taps: Tensor, radius: Tensor, big_r: int, axes_mask: int,
          identity: Tensor | None) -> Tensor:
     """K3 (intensity/blur.py:129-252)."""
-    _require_cuda(src, "blur")
-    src = src.contiguous()
+    src = _batch(src, "blur")
     b, c, i, j, k = src.shape
     dst = torch.empty_like(src)
     scratch = torch.empty_like(src) if (axes_mask & 6) or big_r > WIDE_R else None
-    with torch.cuda.device(src.device):
-        _native.call(
-            "tio_blur", _ptr(src), _ptr(dst), _ptr(scratch), b, c, i, j, k, _ptr(taps),
-            _ptr(radius), int(big_r), int(axes_mask), _ptr(identity), _stream(src),
-        )
+    _launch("tio_blur", src.device, _ptr(src), _ptr(dst), _ptr(scratch), b, c, i, j, k, _ptr(taps),
+            _ptr(radius), int(big_r), int(axes_mask), _ptr(identity))
     return dst
 
 
@@ -438,12 +422,10 @@ def moments(values: Tensor, mask: Tensor | None = None) -> tuple[float, float, f
     """(sum, sum of squares, count) of the selected values of a contiguous fp32 CUDA tensor, fp64
     accumulation on the device, one small D2H read (the reference calls ``.item()`` here too:
     standardize.py:76-77)."""
-    _require_cuda(values, "moments")
-    values = values.contiguous()
+    values = _batch(values, "moments", ndim=None)
     m8 = None if mask is None else mask.expand_as(values).contiguous().to(torch.uint8)
     out = torch.empty(3, dtype=torch.float64, device=values.device)
-    with torch.cuda.device(values.device):
-        _native.call("tio_moments", _ptr(values), _ptr(m8), values.numel(), _ptr(out), _stream(values))
+    _launch("tio_moments", values.device, _ptr(values), _ptr(m8), values.numel(), _ptr(out))
     s, ss, n = out.tolist()
     return s, ss, n
 
@@ -452,8 +434,7 @@ def quantile_neighbours(values: Tensor, qs, mask: Tensor | None = None):
     """For each q in ``qs`` (at most two): the order statistics torch.kthvalue(lower + 1) and
     kthvalue(lower + 2) return, and ``index - lower`` (transforms/_statistics.py:37-45), found by
     an exact radix select on the device.  Returns (values[2m], weights[m], count)."""
-    _require_cuda(values, "quantile_neighbours")
-    values = values.contiguous()
+    values = _batch(values, "quantile_neighbours", ndim=None)
     m8 = None if mask is None else mask.expand_as(values).contiguous().to(torch.uint8)
     qs = np.ascontiguousarray(np.asarray(qs, dtype=np.float64).reshape(-1))
     m = int(qs.shape[0])
@@ -462,9 +443,8 @@ def quantile_neighbours(values: Tensor, qs, mask: Tensor | None = None):
     out = torch.empty(m + 1, dtype=torch.float64, device=dev)
     ws_bytes = _native.lib().tio_quantiles_workspace_bytes()
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        _native.call("tio_quantiles", _ptr(values), _ptr(m8), values.numel(), qs.ctypes.data, m, _ptr(vals),
-                     _ptr(out), out[m:].data_ptr(), _ptr(ws), ws_bytes, _stream(values))
+    _launch("tio_quantiles", dev, _ptr(values), _ptr(m8), values.numel(), qs.ctypes.data, m, _ptr(vals),
+            _ptr(out), out[m:].data_ptr(), _ptr(ws), ws_bytes)
     host = out.tolist()
     return vals.tolist(), host[:m], int(host[m])
 
@@ -474,10 +454,7 @@ def quantiles_batched(values: Tensor, qs, mask: Tensor | None = None):
     taken as ``.float()`` gives them), with any number of quantiles, left on the device: returns
     (values (B, 2m) fp32, weights (B, m) fp64, count (B,) fp64, has_nan (B,) uint8) without a
     host sync (histogram_standardization.py:100-108,279)."""
-    _require_cuda(values, "quantiles_batched")
-    if values.dtype not in RESOLUTION_DTYPE_CODES:
-        raise TypeError(f"quantiles_batched: unsupported dtype {values.dtype}")
-    values = values.contiguous()
+    values = _batch(values, "quantiles_batched", dtypes=IMAGE_DTYPE_CODES, ndim=None)
     b = values.shape[0]
     per_elem = values[0].numel()
     m8 = None if mask is None else mask.expand_as(values).contiguous().to(torch.uint8)
@@ -490,10 +467,8 @@ def quantiles_batched(values: Tensor, qs, mask: Tensor | None = None):
     has_nan = torch.empty(b, dtype=torch.uint8, device=dev)
     ws_bytes = _native.lib().tio_quantiles_batched_workspace_bytes(b, m)
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        _native.call("tio_quantiles_batched", _ptr(values), RESOLUTION_DTYPE_CODES[values.dtype], _ptr(m8), b,
-                     per_elem, qs.ctypes.data, m, _ptr(vals), _ptr(weights), _ptr(count), _ptr(has_nan), _ptr(ws),
-                     ws_bytes, _stream(values))
+    _launch("tio_quantiles_batched", dev, _ptr(values), IMAGE_DTYPE_CODES[values.dtype], _ptr(m8), b, per_elem,
+            qs.ctypes.data, m, _ptr(vals), _ptr(weights), _ptr(count), _ptr(has_nan), _ptr(ws), ws_bytes)
     return vals, weights, count, has_nan
 
 
@@ -504,9 +479,8 @@ def histogram_tables(values: Tensor, weights: Tensor, has_nan: Tensor, landmarks
     b, m = weights.shape
     landmarks = landmarks.to(device=values.device, dtype=torch.float32).contiguous()
     tables = torch.empty((b, 3 * (m - 1)), dtype=torch.float32, device=values.device)
-    with torch.cuda.device(values.device):
-        _native.call("tio_histogram_tables", _ptr(values), _ptr(weights), _ptr(has_nan), _ptr(landmarks), b, m,
-                     _ptr(tables), _stream(values))
+    _launch("tio_histogram_tables", values.device, _ptr(values), _ptr(weights), _ptr(has_nan), _ptr(landmarks), b,
+            m, _ptr(tables))
     return tables
 
 
@@ -514,16 +488,11 @@ def histogram_map(data: Tensor, tables: Tensor, m: int) -> None:
     """In place: each element of the contiguous (B, ...) CUDA tensor ``data`` through its
     piecewise-linear map ``slopes[bin] * x + intercepts[bin]``, bin = torch.bucketize(x, edges),
     computed in fp32 and stored in data's dtype (histogram_standardization.py:302-303)."""
-    _require_cuda(data, "histogram_map")
-    if data.dtype not in RESOLUTION_DTYPE_CODES:
-        raise TypeError(f"histogram_map: unsupported dtype {data.dtype}")
-    if not data.is_contiguous():
-        raise ValueError("histogram_map: data must be contiguous")
+    data = _batch(data, "histogram_map", dtypes=IMAGE_DTYPE_CODES, ndim=None, in_place=True)
     if data.numel() == 0:
         return
-    with torch.cuda.device(data.device):
-        _native.call("tio_histogram_map", _ptr(data), _ptr(data), RESOLUTION_DTYPE_CODES[data.dtype], data.shape[0],
-                     data[0].numel(), _ptr(tables), int(m), _stream(data))
+    _launch("tio_histogram_map", data.device, _ptr(data), _ptr(data), IMAGE_DTYPE_CODES[data.dtype], data.shape[0],
+            data[0].numel(), _ptr(tables), int(m))
 
 
 def rescale(src: Tensor, *, lo: float | None = None, hi: float | None = None, sub=None, div=None, mul=None,
@@ -531,8 +500,7 @@ def rescale(src: Tensor, *, lo: float | None = None, hi: float | None = None, su
     """``((clamp(src, lo, hi) - sub[b]) / div[b]) * mul[b] + add[b]`` over a (B, ...) fp32 batch, each
     step rounded like the reference's separate elementwise ops; omitted steps are skipped.
     ``sub/div/mul/add``: scalars or length-B sequences; ``keep``: length-B, 0 = copy the row."""
-    _require_cuda(src, "rescale")
-    src = src.contiguous()
+    src = _batch(src, "rescale", ndim=None)
     b = src.shape[0]
     flags = (1 if lo is not None else 0)
     tabs = []
@@ -546,10 +514,9 @@ def rescale(src: Tensor, *, lo: float | None = None, hi: float | None = None, su
     keep_np = None if keep is None else np.ascontiguousarray(np.asarray(keep, dtype=np.uint8))
     sub_d, div_d, mul_d, add_d, keep_d = upload(src.device, *tabs, keep_np)
     dst = torch.empty_like(src)
-    with torch.cuda.device(src.device):
-        _native.call("tio_rescale", _ptr(src), _ptr(dst), b, src[0].numel(),
-                     float(lo if lo is not None else 0.0), float(hi if hi is not None else 0.0),
-                     _ptr(sub_d), _ptr(div_d), _ptr(mul_d), _ptr(add_d), _ptr(keep_d), flags, _stream(src))
+    _launch("tio_rescale", src.device, _ptr(src), _ptr(dst), b, src[0].numel(),
+            float(lo if lo is not None else 0.0), float(hi if hi is not None else 0.0),
+            _ptr(sub_d), _ptr(div_d), _ptr(mul_d), _ptr(add_d), _ptr(keep_d), flags)
     return dst
 
 
@@ -572,8 +539,7 @@ def intensity_fused(
     inside the first pass (`tio_intensity_pass1_with_normals`) instead of before it; the
     result is the same bit for bit.
     """
-    _require_cuda(src, "intensity_fused")
-    src = src.contiguous()
+    src = _batch(src, "intensity_fused")
     b, c, i, j, k = src.shape
     if z_replay is not None:
         seed, offset = z_replay
@@ -593,15 +559,13 @@ def intensity_fused(
     si = sj = sk = 0
     if coarse is not None:
         si, sj, sk = coarse.shape[2:]
-    with torch.cuda.device(src.device):
-        _native.call(
-            "tio_intensity_fused", _ptr(src), _ptr(dst), _ptr(scratch), b, c, i, j, k,
-            _ptr(coarse), si, sj, sk, _ptr(bias_identity), int(bool(bias_divide)),
-            _ptr(taps), _ptr(radius), int(big_r), int(axes_mask),
-            _ptr(mean), _ptr(std), _ptr(keep), _ptr(z), _ptr(z2),
-            int(philox_seed) & (2**64 - 1), int(noise_mode), int(bool(rician)),
-            _ptr(gamma), _stream(src),
-        )
+    _launch(
+        "tio_intensity_fused", src.device, _ptr(src), _ptr(dst), _ptr(scratch), b, c, i, j, k,
+        _ptr(coarse), si, sj, sk, _ptr(bias_identity), int(bool(bias_divide)),
+        _ptr(taps), _ptr(radius), int(big_r), int(axes_mask),
+        _ptr(mean), _ptr(std), _ptr(keep), _ptr(z), _ptr(z2),
+        int(philox_seed) & (2**64 - 1), int(noise_mode), int(bool(rician)), _ptr(gamma),
+    )
     return dst
 
 
@@ -614,8 +578,7 @@ def intensity_pass1_with_normals(
     elements [offset, offset + src.numel()) of `randn_mt19937(seed)` shaped like ``src``), from one
     kernel in which the two run side by side on every SM.  Needs table radius <= 6, K % 4 == 0 and
     16-byte aligned data; the library refuses anything else."""
-    _require_cuda(src, "intensity_pass1_with_normals")
-    src = src.contiguous()
+    src = _batch(src, "intensity_pass1_with_normals")
     b, c, i, j, k = src.shape
     n = src.numel()
     if n < 16 or n % 16 or offset % 16 or offset + n > MT_MAX_WORDS:
@@ -629,14 +592,12 @@ def intensity_pass1_with_normals(
     si = sj = sk = 0
     if coarse is not None:
         si, sj, sk = coarse.shape[2:]
-    with torch.cuda.device(src.device):
-        _native.call(
-            "tio_intensity_pass1_with_normals", _ptr(src), _ptr(dst), b, c, i, j, k,
-            _ptr(coarse), si, sj, sk, _ptr(bias_identity), int(bool(bias_divide)),
-            _ptr(taps), _ptr(radius), int(big_r), int(axes_mask),
-            int(seed) & 0xFFFFFFFF, offset, n, _ptr(z), _ptr(table), _ptr(workspace), ws_bytes,
-            _stream(src),
-        )
+    _launch(
+        "tio_intensity_pass1_with_normals", src.device, _ptr(src), _ptr(dst), b, c, i, j, k,
+        _ptr(coarse), si, sj, sk, _ptr(bias_identity), int(bool(bias_divide)),
+        _ptr(taps), _ptr(radius), int(big_r), int(axes_mask),
+        int(seed) & 0xFFFFFFFF, offset, n, _ptr(z), _ptr(table), _ptr(workspace), ws_bytes,
+    )
     return dst, z
 
 
@@ -689,15 +650,17 @@ def mt19937_host_table() -> Tensor:
 
 
 def _mt_table(device: torch.device) -> Tensor:
-    key = (device.type, device.index)
-    table = _mt_device_tables.get(key)
+    """The jump-ahead table on ``device``, copied there once.  Cached by device index: a device
+    without one ("cuda") is the current device, whose table the kernel must read."""
+    index = torch.cuda.current_device() if device.index is None else device.index
+    table = _mt_device_tables.get(index)
     if table is None:
         with _init_lock:
-            table = _mt_device_tables.get(key)
+            table = _mt_device_tables.get(index)
             if table is None:
-                table = mt19937_host_table().to(device)
-                torch.cuda.synchronize(device)  # other threads' streams may read it right away
-                _mt_device_tables[key] = table
+                table = mt19937_host_table().to(torch.device("cuda", index))
+                torch.cuda.synchronize(index)  # other threads' streams may read it right away
+                _mt_device_tables[index] = table
     return table
 
 
@@ -714,9 +677,8 @@ def randn_mt19937(seed: int, offset: int, n: int, device, out: Tensor | None = N
     ws_bytes = lib.tio_randn_mt19937_workspace_bytes(offset, n)
     workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
     table = _mt_table(device)
-    with torch.cuda.device(device):
-        _native.call("tio_randn_mt19937", int(seed) & 0xFFFFFFFF, offset, n, _ptr(z), _ptr(table),
-                     _ptr(workspace), ws_bytes, torch.cuda.current_stream(device).cuda_stream)
+    _launch("tio_randn_mt19937", device, int(seed) & 0xFFFFFFFF, offset, n, _ptr(z), _ptr(table),
+            _ptr(workspace), ws_bytes)
     return z
 
 
@@ -735,6 +697,7 @@ def labels_to_image(labels: Tensor, label_values, means, stds, draw=None) -> Ten
     (default: ascending order, skipping labels whose means and stds are all zero).  Channel 0 is
     read.  One draw of B*I*J*K normals per drawn label is reserved on the device's default CUDA
     generator, as ATen's ``philox_cuda_state`` would hand them out."""
+    # dtype, shape and size are refused before the device is looked at, on any device
     if labels.dtype not in DTYPE_CODES:
         raise TypeError(f"labels_to_image: unsupported label dtype {labels.dtype}")
     if labels.ndim != 5:
@@ -743,7 +706,7 @@ def labels_to_image(labels: Tensor, label_values, means, stds, draw=None) -> Ten
     vox = int(np.prod(labels.shape[2:]))
     numel = b * vox
     tables.check_randn_numel(numel)
-    _require_cuda(labels, "labels_to_image")
+    labels = _batch(labels, "labels_to_image")
     if torch.cuda.is_current_stream_capturing():
         raise RuntimeError("labels_to_image: CUDA-graph capture is not supported (the generator offsets are"
                            " reserved on the host)")
@@ -773,63 +736,46 @@ def labels_to_image(labels: Tensor, label_values, means, stds, draw=None) -> Ten
             gen.set_offset(base + n_draws * counter_offset)
     # draw k starts where the k previous draws left the offset; -1 (all bits set) = not drawn
     offsets = np.where(draw >= 0, base + draw * counter_offset, -1).astype(np.int64)
-    labels = labels.contiguous()
     values_d, mean_d, std_d, offsets_d = upload(device, values, mean, std, offsets) if n else (None,) * 4
-    with torch.cuda.device(device):
-        _native.call("tio_labels_to_image", _ptr(labels), DTYPE_CODES[labels.dtype], c, b, vox, _ptr(values_d), n,
-                     _ptr(mean_d), _ptr(std_d), _ptr(offsets_d), seed & (2**64 - 1), grid_x, _ptr(out),
-                     _stream(labels))
+    _launch("tio_labels_to_image", device, _ptr(labels), DTYPE_CODES[labels.dtype], c, b, vox, _ptr(values_d), n,
+            _ptr(mean_d), _ptr(std_d), _ptr(offsets_d), seed & (2**64 - 1), grid_x, _ptr(out))
     return out
 
 
 # ---- label-map utilities (transforms/label/) ----------------------------------------------------
 
 
-def _label_map(src: Tensor, name: str) -> Tensor:
-    _require_cuda(src, name)
-    if src.dtype not in DTYPE_CODES:
-        raise TypeError(f"{name}: unsupported label dtype {src.dtype}")
-    if src.ndim != 5:
-        raise ValueError(f"{name} expects (B, C, I, J, K), got {tuple(src.shape)}")
-    return src.contiguous()
-
-
 def label_lut(src: Tensor, keys: np.ndarray, values: np.ndarray, *, identity: bool) -> Tensor:
     """``src`` with every element equal to ``keys[i]`` replaced by ``values[i]`` (tables from
     `tables.label_lut`), and every other element kept (``identity``) or set to 0 — the result of
     RemapLabels / RemoveLabels (``clone``) or SequentialLabels (``zeros_like``), one pass."""
-    src = _label_map(src, "label_lut")
+    src = _batch(src, "label_lut", dtypes=DTYPE_CODES)
     dst = torch.empty_like(src)
     n = int(keys.shape[0])
     keys_d, values_d = upload(src.device, keys, values) if n else (None, None)
-    with torch.cuda.device(src.device):
-        _native.call("tio_label_lut", _ptr(src), _ptr(dst), DTYPE_CODES[src.dtype], src.numel(), _ptr(keys_d),
-                     _ptr(values_d), n, int(bool(identity)), _stream(src))
+    _launch("tio_label_lut", src.device, _ptr(src), _ptr(dst), DTYPE_CODES[src.dtype], src.numel(), _ptr(keys_d),
+            _ptr(values_d), n, int(bool(identity)))
     return dst
 
 
 def label_contour(src: Tensor) -> Tensor:
     """(B, C, I, J, K) labels -> fp32 1 where the 3x3x3 minimum of float(v) (-1 outside the volume)
     differs from float(v), else 0 (label/contour.py:52-71)."""
-    src = _label_map(src, "label_contour")
+    src = _batch(src, "label_contour", dtypes=DTYPE_CODES)
     dst = torch.empty(src.shape, dtype=torch.float32, device=src.device)
     if src.numel():
         b, c, i, j, k = src.shape
-        with torch.cuda.device(src.device):
-            _native.call("tio_label_contour", _ptr(src), DTYPE_CODES[src.dtype], b * c, i, j, k, _ptr(dst),
-                         _stream(src))
+        _launch("tio_label_contour", src.device, _ptr(src), DTYPE_CODES[src.dtype], b * c, i, j, k, _ptr(dst))
     return dst
 
 
 def label_range(src: Tensor) -> tuple[int, int]:
     """(min, max) of ``long(v)`` over channel 0 of a non-empty (B, C, I, J, K) batch: one small
     device-to-host read."""
-    src = _label_map(src, "label_range")
+    src = _batch(src, "label_range", dtypes=DTYPE_CODES)
     b, c = src.shape[:2]
     out = torch.empty(2, dtype=torch.int64, device=src.device)
-    with torch.cuda.device(src.device):
-        _native.call("tio_label_range", _ptr(src), DTYPE_CODES[src.dtype], b, c, src[0, 0].numel(), _ptr(out),
-                     _stream(src))
+    _launch("tio_label_range", src.device, _ptr(src), DTYPE_CODES[src.dtype], b, c, src[0, 0].numel(), _ptr(out))
     lo, hi = out.tolist()
     return lo, hi
 
@@ -837,56 +783,38 @@ def label_range(src: Tensor) -> tuple[int, int]:
 def onehot_classes(src: Tensor, num_classes: int) -> Tensor:
     """(B, C, I, J, K) labels -> (B, num_classes, I, J, K) fp32: channel c is ``long(v) == c`` on
     channel 0 of the map (label/one_hot.py:64-68).  The caller checks the classes' range first."""
-    src = _label_map(src, "onehot_classes")
+    src = _batch(src, "onehot_classes", dtypes=DTYPE_CODES)
     b, c = src.shape[:2]
     dst = torch.empty((b, num_classes, *src.shape[2:]), dtype=torch.float32, device=src.device)
-    with torch.cuda.device(src.device):
-        _native.call("tio_onehot_classes", _ptr(src), DTYPE_CODES[src.dtype], b, c, src[0, 0].numel(),
-                     int(num_classes), _ptr(dst), _stream(src))
+    _launch("tio_onehot_classes", src.device, _ptr(src), DTYPE_CODES[src.dtype], b, c, src[0, 0].numel(),
+            int(num_classes), _ptr(dst))
     return dst
 
 
 def channel_argmax(src: Tensor) -> Tensor:
     """(B, C, I, J, K) -> (B, 1, I, J, K) fp32 ``argmax(dim=1, keepdim=True).float()``: the first
     maximum, a NaN counting as the maximum (label/one_hot.py:95-96)."""
-    src = _label_map(src, "channel_argmax")
+    src = _batch(src, "channel_argmax", dtypes=DTYPE_CODES)
     b, c = src.shape[:2]
     dst = torch.empty((b, 1, *src.shape[2:]), dtype=torch.float32, device=src.device)
-    with torch.cuda.device(src.device):
-        _native.call("tio_channel_argmax", _ptr(src), DTYPE_CODES[src.dtype], b, c, src[0, 0].numel(), _ptr(dst),
-                     _stream(src))
+    _launch("tio_channel_argmax", src.device, _ptr(src), DTYPE_CODES[src.dtype], b, c, src[0, 0].numel(), _ptr(dst))
     return dst
 
 
 # ---- resolution changes (spatial/resize.py, spatial/anisotropy.py) ------------------------------
 
-# every label dtype, and fp16 / bf16 / fp64 images, which the kernels compute in fp32 and cast back
-# as the reference's data.float() ... .to(dtype) do (tio_dtype TIO_F16 / TIO_BF16 / TIO_F64)
-RESOLUTION_DTYPE_CODES = {**DTYPE_CODES, torch.float16: 6, torch.bfloat16: 7, torch.float64: 8}
-
-
-def _volume_batch(src: Tensor, name: str) -> Tensor:
-    _require_cuda(src, name)
-    if src.dtype not in RESOLUTION_DTYPE_CODES:
-        raise TypeError(f"{name}: unsupported dtype {src.dtype}")
-    if src.ndim != 5:
-        raise ValueError(f"{name} expects (B, C, I, J, K), got {tuple(src.shape)}")
-    return src.contiguous()
-
-
 def interpolate(src: Tensor, out_shape, idx: np.ndarray, lam: np.ndarray | None) -> Tensor:
     """(B, C, I, J, K) -> (B, C, *out_shape) of src's dtype: ATen's CUDA trilinear
     (align_corners=True; ``lam`` given) or nearest resize of ``src.float()``, cast back, from the
     per-axis tables of `tables.resize_tables` / `tables.anisotropy_shared_tables`, one pass."""
-    src = _volume_batch(src, "interpolate")
+    src = _batch(src, "interpolate", dtypes=IMAGE_DTYPE_CODES)
     b, c, i, j, k = src.shape
     oi, oj, ok = (int(s) for s in out_shape)
     dst = torch.empty((b, c, oi, oj, ok), dtype=src.dtype, device=src.device)
     if src.numel() and dst.numel():
         idx_d, lam_d = upload(src.device, idx, lam)
-        with torch.cuda.device(src.device):
-            _native.call("tio_interpolate", _ptr(src), _ptr(dst), RESOLUTION_DTYPE_CODES[src.dtype], b * c, i, j, k, oi, oj,
-                         ok, _ptr(idx_d), _ptr(lam_d), int(lam is not None), _stream(src))
+        _launch("tio_interpolate", src.device, _ptr(src), _ptr(dst), IMAGE_DTYPE_CODES[src.dtype], b * c, i, j, k,
+                oi, oj, ok, _ptr(idx_d), _ptr(lam_d), int(lam is not None))
     return dst
 
 
@@ -895,7 +823,7 @@ def axis_resample(src: Tensor, axis: np.ndarray, lo: np.ndarray, hi: np.ndarray,
     """Anisotropy's per-instance degradation of a (B, C, I, J, K) batch, one pass: element b is
     resampled along ``axis[b]`` from the (lo, hi, w) rows of `tables.anisotropy_instance_tables`
     (nearest: lo only), or copied when ``axis[b]`` is -1 (anisotropy.py:132-214)."""
-    src = _volume_batch(src, "axis_resample")
+    src = _batch(src, "axis_resample", dtypes=IMAGE_DTYPE_CODES)
     b, c, i, j, k = src.shape
     dst = torch.empty_like(src)
     if src.numel():
@@ -903,10 +831,8 @@ def axis_resample(src: Tensor, axis: np.ndarray, lo: np.ndarray, hi: np.ndarray,
             axis_d, lo_d, hi_d, w_d = upload(src.device, axis, lo, hi, w)
         else:
             (axis_d, lo_d), hi_d, w_d = upload(src.device, axis, lo), None, None
-        with torch.cuda.device(src.device):
-            _native.call("tio_axis_resample", _ptr(src), _ptr(dst), RESOLUTION_DTYPE_CODES[src.dtype], b, c, i, j, k,
-                         _ptr(axis_d), _ptr(lo_d), _ptr(hi_d), _ptr(w_d), int(lo.shape[1]), int(bool(linear)),
-                         _stream(src))
+        _launch("tio_axis_resample", src.device, _ptr(src), _ptr(dst), IMAGE_DTYPE_CODES[src.dtype], b, c, i, j, k,
+                _ptr(axis_d), _ptr(lo_d), _ptr(hi_d), _ptr(w_d), int(lo.shape[1]), int(bool(linear)))
     return dst
 
 
@@ -925,18 +851,14 @@ def clamp(src: Tensor, lo: Tensor | None, hi: Tensor | None) -> Tensor:
     """``torch.clamp(src, lo, hi)`` in one pass (clamp.py:53-56) into a new tensor of the bounds' dtype:
     ``lo`` / ``hi`` are one-element CPU tensors holding the bounds as torch converts them to the
     result dtype (None: no bound), which is src's dtype or fp32 for an integer image."""
-    _require_cuda(src, "clamp")
-    if src.dtype not in RESOLUTION_DTYPE_CODES:
-        raise TypeError(f"clamp: unsupported dtype {src.dtype}")
+    src = _batch(src, "clamp", dtypes=IMAGE_DTYPE_CODES, ndim=None)
     bound = lo if lo is not None else hi
     if bound is None:
         raise ValueError("clamp: no bound")
-    src = src.contiguous()
     dst = torch.empty(src.shape, dtype=bound.dtype, device=src.device)
     (lo_keep, lo_ptr), (hi_keep, hi_ptr) = _scalar_bytes(lo), _scalar_bytes(hi)
-    with torch.cuda.device(src.device):
-        _native.call("tio_clamp", _ptr(src), _ptr(dst), RESOLUTION_DTYPE_CODES[src.dtype],
-                     RESOLUTION_DTYPE_CODES[dst.dtype], src.numel(), lo_ptr, hi_ptr, _stream(src))
+    _launch("tio_clamp", src.device, _ptr(src), _ptr(dst), IMAGE_DTYPE_CODES[src.dtype], IMAGE_DTYPE_CODES[dst.dtype],
+            src.numel(), lo_ptr, hi_ptr)
     del lo_keep, hi_keep
     return dst
 
@@ -947,19 +869,10 @@ def mask(data: Tensor, mask: Tensor, keys: np.ndarray | None, outside: Tensor) -
     to one of ``keys`` (`tables.label_lut`'s keys).  ``outside`` is a one-element CPU tensor of the
     result dtype.  Same dtype: ``data`` is updated in place (only outside voxels are written) and
     returned; fp32 (an integer image): a new fp32 tensor."""
-    _require_cuda(data, "mask")
-    _require_cuda(mask, "mask")
-    if data.dtype not in RESOLUTION_DTYPE_CODES:
-        raise TypeError(f"mask: unsupported dtype {data.dtype}")
-    if mask.dtype == torch.bool:
-        mask = mask.view(torch.uint8)
-    if mask.dtype not in DTYPE_CODES:
-        raise TypeError(f"mask: unsupported mask dtype {mask.dtype}")
-    if data.ndim != 5 or mask.ndim != 4 or mask.shape[0] not in (1, data.shape[1]) or mask.shape[1:] != data.shape[2:]:
+    data = _batch(data, "mask", dtypes=IMAGE_DTYPE_CODES, in_place=True)
+    mask = _batch(mask.view(torch.uint8) if mask.dtype == torch.bool else mask, "mask", dtypes=DTYPE_CODES, ndim=4)
+    if mask.shape[0] not in (1, data.shape[1]) or mask.shape[1:] != data.shape[2:]:
         raise ValueError(f"mask: a {tuple(mask.shape)} mask for a {tuple(data.shape)} batch")
-    if not data.is_contiguous():
-        raise ValueError("mask: data must be contiguous")
-    mask = mask.contiguous()
     b, c = data.shape[:2]
     promote = outside.dtype != data.dtype
     dst = torch.empty(data.shape, dtype=outside.dtype, device=data.device) if promote else data
@@ -967,10 +880,9 @@ def mask(data: Tensor, mask: Tensor, keys: np.ndarray | None, outside: Tensor) -
     (keys_d,) = upload(data.device, keys) if n > 0 else (None,)
     keep, outside_ptr = _scalar_bytes(outside)
     if data.numel():
-        with torch.cuda.device(data.device):
-            _native.call("tio_mask", _ptr(mask), DTYPE_CODES[mask.dtype], mask.shape[0], _ptr(keys_d), n,
-                         _ptr(data), RESOLUTION_DTYPE_CODES[data.dtype], _ptr(dst), RESOLUTION_DTYPE_CODES[dst.dtype],
-                         b, c, data[0, 0].numel(), outside_ptr, _stream(data))
+        _launch("tio_mask", data.device, _ptr(mask), DTYPE_CODES[mask.dtype], mask.shape[0], _ptr(keys_d), n,
+                _ptr(data), IMAGE_DTYPE_CODES[data.dtype], _ptr(dst), IMAGE_DTYPE_CODES[dst.dtype],
+                b, c, data[0, 0].numel(), outside_ptr)
     del keep
     return dst
 
@@ -983,9 +895,7 @@ def swap_patches(data: Tensor, swaps: np.ndarray, patch_size) -> None:
     CUDA batch.  ``swaps``: int32 (1 or B, steps, 8) rows ``ai, aj, ak, bi, bj, bk, kind, 0`` (kind
     SWAP_EXCHANGE for a pair that does not overlap, SWAP_STAGED for one that may, SWAP_NOOP), one
     list for every element or one per element; checked against the volume before any launch."""
-    _require_cuda(data, "swap_patches")
-    if data.ndim != 5 or not data.is_contiguous():
-        raise ValueError(f"swap_patches expects a contiguous (B, C, I, J, K) batch, got {tuple(data.shape)}")
+    data = _batch(data, "swap_patches", in_place=True)
     swaps = np.ascontiguousarray(swaps, dtype=np.int32)
     lists, steps = swaps.shape[:2]
     if steps == 0 or data.numel() == 0:
@@ -996,9 +906,8 @@ def swap_patches(data: Tensor, swaps: np.ndarray, patch_size) -> None:
     stage = None
     if bool((swaps[..., 6] == SWAP_STAGED).any()):
         stage = torch.empty(b * 2 * c * pi * pj * pk * data.element_size(), dtype=torch.uint8, device=data.device)
-    with torch.cuda.device(data.device):
-        _native.call("tio_swap_patches", _ptr(data), data.element_size(), b, c, i, j, k, pi, pj, pk,
-                     swaps.ctypes.data, lists, steps, _ptr(device_list), _ptr(stage), _stream(data))
+    _launch("tio_swap_patches", data.device, _ptr(data), data.element_size(), b, c, i, j, k, pi, pj, pk,
+            swaps.ctypes.data, lists, steps, _ptr(device_list), _ptr(stage))
 
 
 # ---- KeepLargestComponent (label/keep_largest.py) -----------------------------------------------
@@ -1042,7 +951,7 @@ def keep_largest(data: Tensor, labels, background_label, fully_connected: bool) 
         raise ValueError(f"keep_largest: {vox} voxels per element; component roots are 32-bit (at most 2**32 - 1)")
     if b > 65535:
         raise ValueError(f"keep_largest: {b} elements, at most 65535")
-    data = _label_map(data, "keep_largest")
+    data = _batch(data, "keep_largest", dtypes=DTYPE_CODES)
     dtype, dev = data.dtype, data.device
     fill, fill_error = None, None
     try:
@@ -1062,18 +971,16 @@ def keep_largest(data: Tensor, labels, background_label, fully_connected: bool) 
     count = torch.empty_like(roots)
     flags = torch.empty(b, dtype=torch.int32, device=dev)
     code = DTYPE_CODES[dtype]
-    with torch.cuda.device(dev):
-        _native.call("tio_components", _ptr(data), code, b, i, j, k, mode, _ptr(keys_d), n, key, has_key,
-                     int(bool(fully_connected)), _ptr(roots), _ptr(count), _ptr(flags), _stream(data))
-        if mode == KEEP_SEARCH and b * vox:
-            values = torch.empty(b * vox, dtype=dtype, device=dev)
-            n_values = torch.empty(1, dtype=torch.int32, device=dev)
-            _native.call("tio_component_roots", _ptr(data), code, b, vox, _ptr(roots), _ptr(values),
-                         _ptr(n_values), _stream(data))
-            found = values[:int(n_values.item())]  # the one read-back: the distinct labels present
-            keys_d = torch.unique(found).to(torch.float32 if dtype == torch.float32 else torch.int64).contiguous()
-            n = int(keys_d.numel())
-            del values
+    _launch("tio_components", dev, _ptr(data), code, b, i, j, k, mode, _ptr(keys_d), n, key, has_key,
+            int(bool(fully_connected)), _ptr(roots), _ptr(count), _ptr(flags))
+    if mode == KEEP_SEARCH and b * vox:
+        values = torch.empty(b * vox, dtype=dtype, device=dev)
+        n_values = torch.empty(1, dtype=torch.int32, device=dev)
+        _launch("tio_component_roots", dev, _ptr(data), code, b, vox, _ptr(roots), _ptr(values), _ptr(n_values))
+        found = values[:int(n_values.item())]  # the one read-back: the distinct labels present
+        keys_d = torch.unique(found).to(torch.float32 if dtype == torch.float32 else torch.int64).contiguous()
+        n = int(keys_d.numel())
+        del values
     if (labels is None and dtype == torch.float32) or fill_error is not None:
         for bits in flags.tolist():
             if labels is None and bits & KEEP_INF:
@@ -1087,9 +994,8 @@ def keep_largest(data: Tensor, labels, background_label, fully_connected: bool) 
     slots = n if mode != KEEP_VALUE else (65536 if data.element_size() == 2 else 256)
     winner = torch.empty(b * slots, dtype=torch.int64, device=dev)
     keep, fill_ptr = _scalar_bytes(torch.from_numpy(np.ascontiguousarray(fill[:1])))
-    with torch.cuda.device(dev):
-        _native.call("tio_keep_largest", _ptr(data), code, b, vox, mode, _ptr(keys_d), n, key, has_key, _ptr(roots),
-                     _ptr(count), _ptr(winner), fill_ptr, _stream(data))
+    _launch("tio_keep_largest", dev, _ptr(data), code, b, vox, mode, _ptr(keys_d), n, key, has_key, _ptr(roots),
+            _ptr(count), _ptr(winner), fill_ptr)
     del keep
     return data, roots
 
@@ -1107,11 +1013,7 @@ def spike(data: Tensor, spikes: np.ndarray, intensity: np.ndarray) -> Tensor:
     int32 (B, S, 4) rows ``u, v, w, 1`` (frequencies) padded with zeros, ``intensity``: fp32 (B,),
     0 for an element that stays untouched.  Stats, spectrum peak and spike pass stay on the device:
     no host sync."""
-    _require_cuda(data, "spike")
-    if data.dtype not in RESOLUTION_DTYPE_CODES:
-        raise TypeError(f"spike: unsupported dtype {data.dtype}")
-    if data.ndim != 5 or not data.is_contiguous():
-        raise ValueError(f"spike expects a contiguous (B, C, I, J, K) batch, got {tuple(data.shape)}")
+    data = _batch(data, "spike", dtypes=IMAGE_DTYPE_CODES, in_place=True)
     b, c, i, j, k = (int(s) for s in data.shape)
     if max(i, j, k) > SPIKE_MAX_AXIS:
         raise NotImplementedError(
@@ -1129,10 +1031,8 @@ def spike(data: Tensor, spikes: np.ndarray, intensity: np.ndarray) -> Tensor:
     peak = spectrum_peak(data, intensity_d, flags)
     tables_bytes = b * s * (i + j + k) * 8
     tables = torch.empty(tables_bytes, dtype=torch.uint8, device=data.device)
-    with torch.cuda.device(data.device):
-        _native.call("tio_spike", _ptr(data), RESOLUTION_DTYPE_CODES[data.dtype], b, c, i, j, k, _ptr(spikes_d), s,
-                     _ptr(intensity_d), _ptr(total), _ptr(flags), _ptr(peak), _ptr(tables), tables_bytes,
-                     _stream(data))
+    _launch("tio_spike", data.device, _ptr(data), IMAGE_DTYPE_CODES[data.dtype], b, c, i, j, k, _ptr(spikes_d), s,
+            _ptr(intensity_d), _ptr(total), _ptr(flags), _ptr(peak), _ptr(tables), tables_bytes)
     return data
 
 
@@ -1144,9 +1044,8 @@ def spike_stats(data: Tensor, intensity: Tensor) -> tuple[Tensor, Tensor]:
     flags = torch.empty(b * c, dtype=torch.int32, device=data.device)
     ws_bytes = _native.lib().tio_spike_stats_workspace_bytes(b * c)
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=data.device)
-    with torch.cuda.device(data.device):
-        _native.call("tio_spike_stats", _ptr(data), RESOLUTION_DTYPE_CODES[data.dtype], b, c, data[0, 0].numel(),
-                     _ptr(intensity), _ptr(total), _ptr(flags), _ptr(ws), ws_bytes, _stream(data))
+    _launch("tio_spike_stats", data.device, _ptr(data), IMAGE_DTYPE_CODES[data.dtype], b, c, data[0, 0].numel(),
+            _ptr(intensity), _ptr(total), _ptr(flags), _ptr(ws), ws_bytes)
     return total, flags
 
 
@@ -1159,9 +1058,8 @@ def spectrum_peak(data: Tensor, intensity: Tensor, flags: Tensor, workspace_byte
         workspace_bytes = min(b * c, max(1, SPECTRUM_WORKSPACE_BYTES // row_bytes)) * row_bytes
     peak = torch.empty(b * c, dtype=torch.float32, device=data.device)
     ws = torch.empty(workspace_bytes, dtype=torch.uint8, device=data.device)
-    with torch.cuda.device(data.device):
-        _native.call("tio_spectrum_peak", _ptr(data), RESOLUTION_DTYPE_CODES[data.dtype], b, c, i, j, k,
-                     _ptr(intensity), _ptr(flags), _ptr(peak), _ptr(ws), workspace_bytes, _stream(data))
+    _launch("tio_spectrum_peak", data.device, _ptr(data), IMAGE_DTYPE_CODES[data.dtype], b, c, i, j, k,
+            _ptr(intensity), _ptr(flags), _ptr(peak), _ptr(ws), workspace_bytes)
     return peak
 
 
@@ -1176,11 +1074,7 @@ def ghosting(data: Tensor, table: np.ndarray, axis: np.ndarray, active: np.ndarr
     along each element's axis, ``ifft(Hs * fft(x))``.  ``table``: fp32 (B, n_max), element b's
     ``ifftshift(line_mask)`` in its first ``shape[axis[b]]`` entries; ``axis``: (B,) in 0..2;
     ``active``: (B,) bool, False for an element that stays untouched.  No host sync."""
-    _require_cuda(data, "ghosting")
-    if data.dtype not in RESOLUTION_DTYPE_CODES:
-        raise TypeError(f"ghosting: unsupported dtype {data.dtype}")
-    if data.ndim != 5 or not data.is_contiguous():
-        raise ValueError(f"ghosting expects a contiguous (B, C, I, J, K) batch, got {tuple(data.shape)}")
+    data = _batch(data, "ghosting", dtypes=IMAGE_DTYPE_CODES, in_place=True)
     b, c, i, j, k = (int(s) for s in data.shape)
     table = np.ascontiguousarray(table, dtype=np.float32)
     axis = np.ascontiguousarray(axis, dtype=np.int32)
@@ -1201,10 +1095,8 @@ def ghosting(data: Tensor, table: np.ndarray, axis: np.ndarray, active: np.ndarr
         raise ValueError(f"ghosting: table rows of {table.shape[1]} entries for an axis of {longest} points")
     table_d, axis_d, active_d = upload(data.device, table, axis, active)
     flags = torch.empty(b * c, dtype=torch.int32, device=data.device)
-    with torch.cuda.device(data.device):
-        _native.call("tio_ghosting", _ptr(data), RESOLUTION_DTYPE_CODES[data.dtype], b, c, i, j, k, _ptr(table_d),
-                     int(table.shape[1]), _ptr(axis_d), _ptr(active_d), sum(1 << a for a in ghosted), _ptr(flags),
-                     _stream(data))
+    _launch("tio_ghosting", data.device, _ptr(data), IMAGE_DTYPE_CODES[data.dtype], b, c, i, j, k, _ptr(table_d),
+            int(table.shape[1]), _ptr(axis_d), _ptr(active_d), sum(1 << a for a in ghosted), _ptr(flags))
     return data
 
 
@@ -1220,11 +1112,7 @@ def motion(data: Tensor, theta: np.ndarray, active: np.ndarray) -> Tensor:
     fly.  ``theta``: fp32 (B, N, 12), element b's `_affine_matrices` of segment s at ``[b, s - 1]``;
     ``active``: (B,) bool, False for an element that is copied unchanged.  Returns ``data`` itself
     when no element is active.  No host sync."""
-    _require_cuda(data, "motion")
-    if data.dtype not in RESOLUTION_DTYPE_CODES:
-        raise TypeError(f"motion: unsupported dtype {data.dtype}")
-    if data.ndim != 5 or not data.is_contiguous():
-        raise ValueError(f"motion expects a contiguous (B, C, I, J, K) batch, got {tuple(data.shape)}")
+    data = _batch(data, "motion", dtypes=IMAGE_DTYPE_CODES, in_place=True)
     b, c, i, j, k = (int(s) for s in data.shape)
     theta = np.ascontiguousarray(theta, dtype=np.float32)
     active = np.ascontiguousarray(active, dtype=np.uint8)
@@ -1242,7 +1130,6 @@ def motion(data: Tensor, theta: np.ndarray, active: np.ndarray) -> Tensor:
     theta_d, active_d = upload(data.device, theta, active)
     out = torch.empty_like(data)
     flags = torch.empty(b * c, dtype=torch.int32, device=data.device)
-    with torch.cuda.device(data.device):
-        _native.call("tio_motion", _ptr(data), _ptr(out), RESOLUTION_DTYPE_CODES[data.dtype], b, c, i, j, k, segments,
-                     _ptr(theta_d), _ptr(active_d), _ptr(flags), _stream(data))
+    _launch("tio_motion", data.device, _ptr(data), _ptr(out), IMAGE_DTYPE_CODES[data.dtype], b, c, i, j, k,
+            segments, _ptr(theta_d), _ptr(active_d), _ptr(flags))
     return out

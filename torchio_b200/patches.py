@@ -324,7 +324,7 @@ class PatchAggregator:
         staged = []
         for key, tensor in tensors.items():
             tensor = tensor if tensor.device == device else tensor.to(device)
-            ops._require_cuda(tensor, "aggregate_patches")
+            ops._check(tensor, "aggregate_patches")
             staged.append((key, tensor, tables[key]))
         for key, tensor, table in staged:
             if key not in self._outputs:
