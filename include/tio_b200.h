@@ -107,6 +107,42 @@ uint64_t tio_launch_count(void);
  * src and dst must not alias.
  */
 size_t tio_resample_workspace_bytes(int B, int OI, int OJ, int OK);
+
+/*
+ * B-spline interpolation of orders 2-7 (image_interpolation / label_interpolation /
+ * one_hot_label_interpolation "quadratic" ... "seventh"): the reference's
+ *   interpol.grid_pull(data.float(), voxel_grid, interpolation=order, bound="dct2",
+ *                      extrapolate=False, prefilter=True)
+ * (transforms/spatial/spatial.py:1734-1761, 1860-1878), in two steps.
+ *
+ * tio_bspline_prefilter: coeff (B, C, I, J, K) fp32 = the interpolating B-spline coefficients of
+ *   src (B, C, I, J, K) of `dtype` (TIO_F32 .. TIO_I64) under the half-sample-symmetric (dct2)
+ *   boundary, per (b, c) volume: one pass per axis longer than 1 (at most three launches).
+ *   Elements whose flags[b] has TIO_FLAG_PASSTHROUGH are skipped (flags may be NULL).  coeff may
+ *   be src itself when dtype is TIO_F32 (in place); it must not overlap src otherwise.  A volume
+ *   of 1 x 1 x 1 voxels is copied (converted to fp32) unless coeff is src.  Axes of up to 51199
+ *   voxels: a CTA stages whole lines in 200 KiB of shared memory (32 lines per CTA up to 1599
+ *   voxels, fewer above); a longer axis is refused.
+ *
+ * tio_bspline_resample: dst (B, C, OI, OJ, OK) of `dtype` = the spline of coeff at the input-voxel
+ *   coordinates tio_resample computes from mat / cp / flags / spacings / affine_first (same
+ *   arguments, same fp32 arithmetic) before its [-1, 1] normalisation.  A voxel with any
+ *   coordinate outside (-0.05, n - 1 + 0.05) of its axis is 0; the sum is cast to `dtype` by
+ *   truncation, as Tensor.to.  Passthrough elements copy src (the data coeff was made from)
+ *   bit-exactly.  One launch.  dst must not overlap coeff or src.
+ *
+ * Both validate every argument before launching (order outside 2-7, null pointers, forbidden
+ * aliasing: non-zero return, tio_last_error) and allocate nothing.
+ */
+int tio_bspline_prefilter(const void* src, int dtype, float* coeff, const uint8_t* flags,
+                          int B, int C, int I, int J, int K, int order, void* stream);
+int tio_bspline_resample(const float* coeff, const void* src, void* dst, int dtype,
+                         int B, int C, int I, int J, int K,
+                         int OI, int OJ, int OK,
+                         const float* mat, const float* cp, const uint8_t* flags,
+                         int ni, int nj, int nk,
+                         const float* spacing_in, const float* spacing_out,
+                         int affine_first, int order, void* stream);
 int tio_resample(const void* src, void* dst, int dtype,
                  int B, int C, int I, int J, int K,
                  int OI, int OJ, int OK,

@@ -106,36 +106,38 @@ __device__ __forceinline__ T label_pv_pick(const T tap[8], const float w[8], con
   return (total > 0.5f) ? best : pad;
 }
 
-// General per-thread column: walks output planes [oi0, oi_end) at (oj, ok),
-// gathering straight from global memory with exact ATen rounding everywhere
-// (bit-exact with oracle/c/tio_oracle.c for every dtype and mode).
-template <typename T, int MODE, bool HAS_CP, bool HAS_FILL>
-__device__ __forceinline__ void general_column(const ResampleArgs& a, const int b, const bool elastic,
-                                               const float* g, const T* __restrict__ src,
-                                               T* __restrict__ dst, const int64_t n_in,
-                                               const int64_t n_out, const int oi0,
-                                               const int oi_end, const int oj, const int ok) {
+// The reference's fp32 input-voxel coordinates q = voxel_grid (spatial.py:1504-1579) of the output
+// voxels of one (oj, ok) column, walked along I: the affine row of each axis, with the control-point
+// displacement d = lerp_I(lerp_J(lerp_K(cp))) added before (affine_first) or after it.  The two
+// inner lerp levels stay in registers across the walk and are recomputed only when the walk enters
+// a new control-grid cell.  Shared by K1 and the B-spline pull, so both sample at the same points.
+template <bool HAS_CP>
+struct ColumnCoords {
   float m[12];
-#pragma unroll
-  for (int t = 0; t < 12; ++t) m[t] = a.mat[b * 12 + t];
-
-  // per-thread J/K lerp setup for the displacement field
   LerpAxis lj, lk;
   int64_t o00 = 0, o01 = 0, o10 = 0, o11 = 0;  // (j0|j1, k0|k1) offsets in cp, x3
-  if (HAS_CP && elastic) {
-    lj = lerp_axis(a.sc_j, a.nj, oj);
-    lk = lerp_axis(a.sc_k, a.nk, ok);
-    o00 = ((int64_t)lj.i0 * a.nk + lk.i0) * 3;
-    o01 = ((int64_t)lj.i0 * a.nk + lk.i1) * 3;
-    o10 = ((int64_t)lj.i1 * a.nk + lk.i0) * 3;
-    o11 = ((int64_t)lj.i1 * a.nk + lk.i1) * 3;
-  }
-  const int plane = a.nj * a.nk * 3;
-  int cur_i0 = -1, cur_i1 = -1;
+  int plane, cur_i0 = -1, cur_i1 = -1;
   float r_lo[3] = {0.f, 0.f, 0.f}, r_hi[3] = {0.f, 0.f, 0.f};
+  float pj, pk;
+  bool elastic;
 
-  const float pj = (float)oj, pk = (float)ok;
-  for (int oi = oi0; oi < oi_end; ++oi) {
+  __device__ __forceinline__ ColumnCoords(const ResampleArgs& a, const int b, const bool elastic_,
+                                          const int oj, const int ok)
+      : plane(a.nj * a.nk * 3), pj((float)oj), pk((float)ok), elastic(elastic_) {
+#pragma unroll
+    for (int t = 0; t < 12; ++t) m[t] = a.mat[b * 12 + t];
+    if (HAS_CP && elastic) {
+      lj = lerp_axis(a.sc_j, a.nj, oj);
+      lk = lerp_axis(a.sc_k, a.nk, ok);
+      o00 = ((int64_t)lj.i0 * a.nk + lk.i0) * 3;
+      o01 = ((int64_t)lj.i0 * a.nk + lk.i1) * 3;
+      o10 = ((int64_t)lj.i1 * a.nk + lk.i0) * 3;
+      o11 = ((int64_t)lj.i1 * a.nk + lk.i1) * 3;
+    }
+  }
+
+  // q of output plane oi; `g` is the element's control grid (shared or global memory)
+  __device__ __forceinline__ void at(const ResampleArgs& a, const float* g, const int oi, float q[3]) {
     const float pi = (float)oi;
     float d[3] = {0.f, 0.f, 0.f};
     if (HAS_CP && elastic) {
@@ -158,8 +160,6 @@ __device__ __forceinline__ void general_column(const ResampleArgs& a, const int 
 #pragma unroll
       for (int ax = 0; ax < 3; ++ax) d[ax] = lerp2(li.l0, r_lo[ax], li.l1, r_hi[ax]);
     }
-
-    float q[3];
     if (!(HAS_CP && elastic)) {
 #pragma unroll
       for (int ax = 0; ax < 3; ++ax) q[ax] = affine_row(m + 4 * ax, pi, pj, pk);
@@ -174,6 +174,22 @@ __device__ __forceinline__ void general_column(const ResampleArgs& a, const int 
 #pragma unroll
       for (int ax = 0; ax < 3; ++ax) q[ax] = affine_row(m + 4 * ax, e0, e1, e2);
     }
+  }
+};
+
+// General per-thread column: walks output planes [oi0, oi_end) at (oj, ok),
+// gathering straight from global memory with exact ATen rounding everywhere
+// (bit-exact with oracle/c/tio_oracle.c for every dtype and mode).
+template <typename T, int MODE, bool HAS_CP, bool HAS_FILL>
+__device__ __forceinline__ void general_column(const ResampleArgs& a, const int b, const bool elastic,
+                                               const float* g, const T* __restrict__ src,
+                                               T* __restrict__ dst, const int64_t n_in,
+                                               const int64_t n_out, const int oi0,
+                                               const int oi_end, const int oj, const int ok) {
+  ColumnCoords<HAS_CP> coords(a, b, elastic, oj, ok);
+  for (int oi = oi0; oi < oi_end; ++oi) {
+    float q[3];
+    coords.at(a, g, oi, q);
     float u[3];
 #pragma unroll
     for (int ax = 0; ax < 3; ++ax) u[ax] = renormalise(q[ax], a.nm1[ax], a.sm1[ax]);

@@ -228,6 +228,45 @@ def resample(
     return dst
 
 
+def bspline_prefilter(src: Tensor, order: int, flags: Tensor | None = None, *, in_place: bool = False) -> Tensor:
+    """(B,C,I,J,K) -> fp32 interpolating B-spline coefficients of ``order`` (2-7) under the dct2
+    boundary, the prefilter of ``interpol.grid_pull(..., bound="dct2", prefilter=True)``
+    (spatial/spatial.py:1734-1761, 1860-1878).  ``in_place`` (fp32 ``src`` only) overwrites ``src``
+    with them.  Elements flagged passthrough are left as they are."""
+    src = _batch(src, "bspline_prefilter", dtypes=DTYPE_CODES, in_place=in_place)
+    if in_place and src.dtype != torch.float32:
+        raise TypeError(f"bspline_prefilter: in_place needs a float32 tensor, got {src.dtype}")
+    coeff = src if in_place else torch.empty(src.shape, dtype=torch.float32, device=src.device)
+    _launch("tio_bspline_prefilter", src.device, _ptr(src), DTYPE_CODES[src.dtype], _ptr(coeff), _ptr(flags),
+            *src.shape, int(order))
+    return coeff
+
+
+def bspline_resample(
+    coeff: Tensor, src: Tensor, mat: Tensor, cp: Tensor | None, flags: Tensor | None,
+    spacing_in, spacing_out, *, affine_first: bool, order: int, out_shape=None,
+) -> Tensor:
+    """The B-spline of ``coeff`` (from `bspline_prefilter`) at K1's sampling coordinates, 0 outside
+    (-0.05, n - 1 + 0.05), cast to ``src.dtype``; passthrough elements copy ``src``.  Geometry
+    arguments as `resample`."""
+    src = _batch(src, "bspline_resample", dtypes=DTYPE_CODES)
+    _check(coeff, "bspline_resample", dtypes=(torch.float32,))
+    if coeff.shape != src.shape or not coeff.is_contiguous():
+        raise ValueError(f"bspline_resample: coeff must be contiguous of shape {tuple(src.shape)}")
+    b, c, i, j, k = src.shape
+    oi, oj, ok = (i, j, k) if out_shape is None else out_shape
+    dst = torch.empty((b, c, oi, oj, ok), dtype=src.dtype, device=src.device)
+    ni = nj = nk = 0
+    if cp is not None:
+        ni, nj, nk = cp.shape[1:4]
+    sp_in = np.asarray(spacing_in, dtype=np.float32)
+    sp_out = np.asarray(spacing_out, dtype=np.float32)
+    _launch("tio_bspline_resample", src.device, _ptr(coeff), _ptr(src), _ptr(dst), DTYPE_CODES[src.dtype],
+            b, c, i, j, k, oi, oj, ok, _ptr(mat), _ptr(cp), _ptr(flags), ni, nj, nk,
+            sp_in.ctypes.data, sp_out.ctypes.data, int(bool(affine_first)), int(order))
+    return dst
+
+
 def _label_table(labels: Tensor, dtype: torch.dtype, device: torch.device) -> Tensor:
     return labels.to(device=device, dtype=torch.float32 if dtype == torch.float32 else torch.int64).contiguous()
 

@@ -8,11 +8,15 @@ three small tables and runs ONE fused CUDA pass per image
 (`ops.resample`, K1) instead of materialising a sampling grid and calling
 ``grid_sample`` twice (spatial.py:1110-1272, 1504-1857).
 
-Supported natively: interpolation orders 0-1 (``"nearest"``/``"linear"``) and the partial-volume
-``label_interpolation="label"``; ``target=None``, a concrete ``(shape, affine)`` space, an
-image, an image name or (random) spacings; ``antialias``; fills ``"minimum"``, ``"mean"``,
-``"otsu"`` or numeric.  Raise NotImplementedError: B-spline orders >= 2 (the reference delegates
-them to ``torch-interpol``, which is neither vendored nor installed) and file-path targets.
+Supported natively: interpolation orders 0-1 (``"nearest"``/``"linear"``) through K1, B-spline
+orders 2-7 (``"quadratic"`` ... ``"seventh"``) through a separable prefilter and an (n+1)^3-tap pull
+at K1's sampling coordinates (the reference's ``interpol.grid_pull(bound="dct2",
+extrapolate=False, prefilter=True)``, spatial.py:1734-1761, 1860-1878), and the partial-volume
+``label_interpolation="label"`` with any one-hot order; ``target=None``, a concrete
+``(shape, affine)`` space, an image, an image name or (random) spacings; ``antialias``; fills
+``"minimum"``, ``"mean"``, ``"otsu"`` or numeric (orders 2-7 ignore them, as the reference does:
+their out-of-bounds voxels are 0; their prefilter refuses an axis longer than 51199 voxels).
+Raise NotImplementedError: file-path targets.
 """
 
 from __future__ import annotations
@@ -771,27 +775,29 @@ def _fill_tensor(data: Tensor, is_label: bool, pad_value, pad_label):
     return torch.full((c,), value, dtype=torch.float32, device=data.device)
 
 
-def _resample_label_pv(data, resample, *, antialias, a_in, a_out, one_hot_interpolation, pad_label):
+def _resample_label_pv(data, resample, spline, *, antialias, a_in, a_out, one_hot_interpolation, pad_label):
     """``label_interpolation="label"`` (spatial.py:1275-1389).  ``resample(tensor, mode, fill, exact)``
-    runs K1 with the call's geometry.
+    runs K1 with the call's geometry, ``spline(tensor, order, in_place)`` the B-spline pull of order
+    2-7 (`_spline`).
 
     C == 1, linear, no anti-aliasing: the fused TIO_LABEL_PV mode (no one-hot channels in HBM).
     C == 1 otherwise: one-hot channels -> [blur] -> K1 with the reference's exact coordinate chain
-    (argmax ties and the 0.5 threshold are decided by the last bit) -> argmax / pad label.
+    (argmax ties and the 0.5 threshold are decided by the last bit), or the B-spline prefilter in
+    place and pull -> argmax / pad label.
     C > 1: the channels are sampled as they are, zero padding, floating-point result."""
-    if one_hot_interpolation not in ("nearest", "linear"):
-        raise NotImplementedError(
-            f'one_hot_label_interpolation "{one_hot_interpolation}" is not implemented in torchio_b200'
-            " (orders 0-1 only)")
-    mode = ops.NEAREST if one_hot_interpolation == "nearest" else ops.LINEAR
+    order = _ORDERS[one_hot_interpolation]
+    mode = ops.NEAREST if order == 0 else ops.LINEAR
     if data.shape[1] > 1:
         smoothed = data if data.dtype == torch.float32 else data.float()
         if antialias:
             smoothed = _antialias(smoothed, a_in, a_out)
-        sampled = resample(smoothed, mode, None, True)
+        if order >= 2:  # in place only on a tensor made here
+            sampled = spline(smoothed, order, smoothed is not data)
+        else:
+            sampled = resample(smoothed, mode, None, True)
         return sampled.to(data.dtype) if data.dtype.is_floating_point else sampled
     native = data if data.dtype in ops.DTYPE_CODES else data.float()
-    if not antialias and mode == ops.LINEAR:
+    if not antialias and order == 1:
         pad = torch.full((1,), float(pad_label), dtype=torch.float32, device=data.device)
         out = resample(native, ops.LABEL_PV, pad, True)
     else:
@@ -799,7 +805,10 @@ def _resample_label_pv(data, resample, *, antialias, a_in, a_out, one_hot_interp
         one_hot = ops.onehot(native, labels)
         if antialias:
             one_hot = _antialias(one_hot, a_in, a_out)
-        sampled = resample(one_hot, mode, None, True)
+        if order >= 2:
+            sampled = spline(one_hot, order, True)
+        else:
+            sampled = resample(one_hot, mode, None, True)
         out = ops.label_argmax(sampled, labels, float(pad_label), native.dtype)
     return out if out.dtype == data.dtype else out.to(data.dtype)
 
@@ -826,7 +835,8 @@ def _apply_spatial(batch, names, target_space, geometry, *, affine_first, image_
         for name in names:
             ib = batch.images[name]
             is_label = issubclass(ib._image_class, LabelMap)
-            if is_label and label_interpolation == LABEL_INTERPOLATION:
+            interp = label_interpolation if is_label else image_interpolation
+            if interp == LABEL_INTERPOLATION or _ORDERS[interp] >= 2:  # no fill
                 continue
             native = ib.data if ib.data.dtype in ops.DTYPE_CODES else ib.data.float()
             info.cache[("fill", info.step, name)] = _fill_tensor(native, is_label, default_pad_value,
@@ -838,6 +848,18 @@ def _apply_spatial(batch, names, target_space, geometry, *, affine_first, image_
     device = first.data.device
     mat_d, cp_d, flags_d = ops.upload(device, packed.mat, packed.cp, packed.flags)
     box_hint = _box_hint(packed, a_in.spacing, a_out.spacing, out_shape)
+    target_shape = None if target_space is None else out_shape
+
+    def spline(tensor, order, in_place, source=None):
+        """B-spline of ``order`` through the call's geometry: coefficients of ``tensor`` (over it
+        when ``in_place``), passthrough elements copied from ``source`` (default ``tensor``, whose
+        passthrough elements the prefilter leaves as they are)."""
+        coeff = ops.bspline_prefilter(tensor, order, flags_d, in_place=in_place)
+        return ops.bspline_resample(
+            coeff, tensor if source is None else source, mat_d, cp_d, flags_d, a_in.spacing, a_out.spacing,
+            affine_first=affine_first, order=order, out_shape=target_shape)
+
+    keep_original = set(packed.passthrough)
     for name in names:
         ib = batch.images[name]
         is_label = issubclass(ib._image_class, LabelMap)
@@ -847,19 +869,24 @@ def _apply_spatial(batch, names, target_space, geometry, *, affine_first, image_
             def run(tensor, mode, fill, exact):
                 return ops.resample(
                     tensor, mat_d, cp_d, flags_d, a_in.spacing, a_out.spacing, affine_first=affine_first,
-                    mode=mode, fill=fill, out_shape=None if target_space is None else out_shape,
-                    box_hint=box_hint, exact_coords=exact)
+                    mode=mode, fill=fill, out_shape=target_shape, box_hint=box_hint, exact_coords=exact)
             ib.data = _resample_label_pv(
-                data, run, antialias=antialias, a_in=a_in, a_out=a_out,
+                data, run, spline, antialias=antialias, a_in=a_in, a_out=a_out,
                 one_hot_interpolation=one_hot_label_interpolation, pad_label=default_pad_label)
-            keep_original = set(packed.passthrough)
             ib.affines[:] = [ib.affines[i] if i in keep_original else a_out.clone() for i in range(b)]
             continue
-        if interp not in ("nearest", "linear"):
-            raise NotImplementedError(
-                f'interpolation "{interp}" is not implemented in torchio_b200 (orders 0-1 only)'
-            )
         native = data if data.dtype in ops.DTYPE_CODES else data.float()
+        order = _ORDERS[interp]
+        if order >= 2:  # data.float() -> [blur] -> grid_pull -> .to(dtype); no fill (spatial.py:1734-1761)
+            smoothed = _antialias(native, a_in, a_out) if antialias and not is_label else native
+            out = spline(smoothed, order, False, native)
+            out = out if out.dtype == data.dtype else out.to(data.dtype)
+            if keep_original and data.dtype not in ops.DTYPE_CODES:  # native rounded them to fp32
+                rows = torch.tensor(sorted(keep_original), device=device)
+                out[rows] = data[rows]
+            ib.data = out
+            ib.affines[:] = [ib.affines[i] if i in keep_original else a_out.clone() for i in range(b)]
+            continue
         if info is None:
             fill = _fill_tensor(native, is_label, default_pad_value, default_pad_label)
         else:  # streamed: derived from batch element 0 when the first slice came through
@@ -869,11 +896,10 @@ def _apply_spatial(batch, names, target_space, geometry, *, affine_first, image_
         out = ops.resample(
             native, mat_d, cp_d, flags_d, a_in.spacing, a_out.spacing,
             affine_first=affine_first, mode=ops.NEAREST if interp == "nearest" else ops.LINEAR,
-            fill=fill, out_shape=None if target_space is None else out_shape,
+            fill=fill, out_shape=target_shape,
             box_hint=box_hint,
         )
         ib.data = out if out.dtype == data.dtype else out.to(data.dtype)
-        keep_original = set(packed.passthrough)
         ib.affines[:] = [
             ib.affines[i] if i in keep_original else a_out.clone() for i in range(b)
         ]
