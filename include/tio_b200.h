@@ -686,6 +686,33 @@ int tio_aggregate_patches(const void* patches, void* out, void* counts, int dtyp
 int tio_aggregate_finish(const void* out, const void* counts, void* dst, int dtype, int C, int64_t vox,
                          void* stream);
 
+/*
+ * PCA (intensity/pca.py of the reference: per element, A = (voxels x channels) float(x) minus its
+ * channel means, torch.pca_lowrank(A, q), A @ V, whitening, normalising and the values_range map).
+ * `src` is a contiguous (B, C, vox) batch of any tio_dtype, read as `data.float()`; B <= 65535.  The
+ * three passes below are the only reads of the volume; the C x q algebra between them runs on the
+ * host.  Both reductions add fixed-order block partials (no float atomics): the same input gives the
+ * same bits.
+ *
+ * tio_pca_workspace_bytes: device scratch that tio_pca_mean and tio_pca_gram_apply need for this
+ * shape (the larger of the two); one workspace serves both passes of a stream in turn.
+ *
+ * tio_pca_mean: mean[b * C + c] (device fp64) = the mean of float(x) over the element's voxels.
+ *
+ * tio_pca_gram_apply: out[b][c][k] (device fp64) = sum_v d[v][c] (sum_c' d[v][c'] w[b][c'][k]), that
+ * is G W with G = A^T A, for d = float(x) - mean in fp64; w is device fp64 [B][C][q], 1 <= q <= 6144.
+ *
+ * tio_pca_project: out[b][k][v] (device fp32) = sum_c (float(x) - (float)mean) * coef[b][c][k] +
+ * offset, in fp32, clamped to [0, 1] when `clip` (NaN stays NaN); coef is device fp32 [B][C][q].
+ */
+size_t tio_pca_workspace_bytes(int B, int C, int q, int64_t vox);
+int tio_pca_mean(const void* src, int dtype, int B, int C, int64_t vox, double* mean, void* workspace,
+                 size_t workspace_bytes, void* stream);
+int tio_pca_gram_apply(const void* src, int dtype, int B, int C, int64_t vox, int q, const double* mean,
+                       const double* w, double* out, void* workspace, size_t workspace_bytes, void* stream);
+int tio_pca_project(const void* src, int dtype, int B, int C, int64_t vox, int q, const double* mean,
+                    const float* coef, float offset, int clip, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

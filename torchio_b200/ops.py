@@ -1172,3 +1172,56 @@ def motion(data: Tensor, theta: np.ndarray, active: np.ndarray) -> Tensor:
     _launch("tio_motion", data.device, _ptr(data), _ptr(out), IMAGE_DTYPE_CODES[data.dtype], b, c, i, j, k,
             segments, _ptr(theta_d), _ptr(active_d), _ptr(flags))
     return out
+
+
+# ---- PCA (intensity/pca.py) ---------------------------------------------------------------------
+
+def pca_workspace(data: Tensor, q: int) -> Tensor:
+    """Device scratch of `tio_pca_mean` and `tio_pca_gram_apply` for a (B, C, ...) batch and ``q``
+    or one column; one workspace serves every pass of a call."""
+    b, c = int(data.shape[0]), int(data.shape[1])
+    vox = data[0, 0].numel()
+    nbytes = max(_native.lib().tio_pca_workspace_bytes(b, c, cols, vox) for cols in (q, 1))
+    return torch.empty(nbytes, dtype=torch.uint8, device=data.device)
+
+
+def pca_mean(data: Tensor, workspace: Tensor) -> Tensor:
+    """fp64 (B, C) channel means of float(x) for a contiguous (B, C, I, J, K) CUDA batch of any image
+    dtype (pca.py:105), added in a fixed order."""
+    data = _batch(data, "pca_mean", dtypes=IMAGE_DTYPE_CODES, in_place=True)
+    b, c = int(data.shape[0]), int(data.shape[1])
+    mean = torch.empty(b, c, dtype=torch.float64, device=data.device)
+    _launch("tio_pca_mean", data.device, _ptr(data), IMAGE_DTYPE_CODES[data.dtype], b, c, data[0, 0].numel(),
+            _ptr(mean), _ptr(workspace), workspace.numel())
+    return mean
+
+
+def pca_gram_apply(data: Tensor, mean: Tensor, w: np.ndarray, workspace: Tensor) -> Tensor:
+    """fp64 (B, C, q) products G W of each element, G = A^T A for A = float(x) - mean (voxels x
+    channels), from one read of the batch; ``w``: (B, C, q) float64 on the host, uploaded."""
+    data = _batch(data, "pca_gram_apply", dtypes=IMAGE_DTYPE_CODES, in_place=True)
+    b, c = int(data.shape[0]), int(data.shape[1])
+    w = np.ascontiguousarray(w, dtype=np.float64)
+    if w.ndim != 3 or w.shape[:2] != (b, c) or w.shape[2] < 1:
+        raise ValueError(f"pca_gram_apply: w {w.shape} for a batch of {b} x {c} channels")
+    (w_d,) = upload(data.device, w)
+    out = torch.empty(w.shape, dtype=torch.float64, device=data.device)
+    _launch("tio_pca_gram_apply", data.device, _ptr(data), IMAGE_DTYPE_CODES[data.dtype], b, c, data[0, 0].numel(),
+            int(w.shape[2]), _ptr(mean), _ptr(w_d), _ptr(out), _ptr(workspace), workspace.numel())
+    return out
+
+
+def pca_project(data: Tensor, mean: Tensor, coef: np.ndarray, offset: float, clip: bool) -> Tensor:
+    """fp32 (B, q, I, J, K): ``sum_c (float(x_c) - mean_c) coef[b, c, k] + offset`` in fp32, clamped
+    to [0, 1] when ``clip`` (pca.py:111-130 with the scales folded into ``coef``: (B, C, q))."""
+    data = _batch(data, "pca_project", dtypes=IMAGE_DTYPE_CODES, in_place=True)
+    b, c = int(data.shape[0]), int(data.shape[1])
+    coef = np.ascontiguousarray(coef, dtype=np.float32)
+    if coef.ndim != 3 or coef.shape[:2] != (b, c) or coef.shape[2] < 1:
+        raise ValueError(f"pca_project: coef {coef.shape} for a batch of {b} x {c} channels")
+    q = int(coef.shape[2])
+    (coef_d,) = upload(data.device, coef)
+    out = torch.empty((b, q, *data.shape[2:]), dtype=torch.float32, device=data.device)
+    _launch("tio_pca_project", data.device, _ptr(data), IMAGE_DTYPE_CODES[data.dtype], b, c, data[0, 0].numel(), q,
+            _ptr(mean), _ptr(coef_d), float(offset), int(bool(clip)), _ptr(out))
+    return out

@@ -13,11 +13,12 @@ from .resolution import Anisotropy, Resize
 from .spatial import Affine, ElasticDeformation, Resample, Spatial
 from .ghosting import Ghosting
 from .motion import Motion
+from .pca import PCA
 from .spike import Spike
 
 __all__ = [
     "Affine", "Anisotropy", "AppliedTransform", "BiasField", "Blur", "Clamp", "Compose", "Contour", "CopyAffine", "Crop", "CropOrPad", "ElasticDeformation", "EnsureShapeMultiple",
-    "Flip", "Gamma", "Ghosting", "HistogramStandardization", "IntensityTransform", "KeepLargestComponent", "LabelsToImage", "Mask", "Motion", "Noise", "Normalize", "OneHot", "Pad", "RemapLabels",
+    "Flip", "Gamma", "Ghosting", "HistogramStandardization", "IntensityTransform", "KeepLargestComponent", "LabelsToImage", "Mask", "Motion", "Noise", "Normalize", "OneHot", "PCA", "Pad", "RemapLabels",
     "RemoveLabels", "Reorient", "Resample", "Resize", "RescaleIntensity", "SequentialLabels", "Spatial",
     "SpatialTransform", "Spike", "Standardize", "Swap", "ToReferenceSpace", "Transform", "Transpose", "ZNormalization",
     "apply_inverse_transform", "compute_histogram_landmarks", "execution_device", "get_inverse_transform",

@@ -106,6 +106,16 @@ def staged_derived(name: str, source: str) -> None:
         staging.derive(name, source)
 
 
+def staged_source_device(name: str, data: Tensor) -> torch.device:
+    """The device image ``name`` had before the call staged it on the execution device (a host
+    batch's CPU), or ``data``'s device when it was not staged: random draws the reference makes on
+    the data's device come from that device's generator."""
+    staging = getattr(_staging_local, "active", None)
+    if staging is not None and name in staging.origin:
+        return staging.origin[name][0]
+    return data.device
+
+
 class _Staging:
     """Move a CPU batch to the execution device and back, preserving pinning.  Images a transform
     adds during the call are brought back like the image they were derived from."""
