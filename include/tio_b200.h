@@ -151,6 +151,26 @@ int tio_resample(const void* src, void* dst, int dtype,
                  const float* spacing_in, const float* spacing_out,
                  int affine_first, int mode, const float* fill, int box_hint,
                  void* workspace, size_t workspace_bytes, void* stream);
+/*
+ * tio_resample with a box edge per batch element: fp32 + TIO_LINEAR (no TIO_EXACT_COORDS),
+ * box_hint >= 0 and a workspace.  `elems` (device int[B]) lists every batch element once, and
+ * `runs` (host int[2 * n_runs]: count, edge) splits that list into runs of ascending edges
+ * (20 / 22 / 24 / 28 / 32, 1 <= n_runs <= 5, counts summing to B).  Each run is one bounds
+ * pre-pass and one tile launch over its elements with that box, writing its elements' output.
+ * A tile takes the staged box when its pre-image fits its run's box, so a caller that wants the
+ * output of tio_resample(..., box_hint = E) picks for each element an edge that holds every
+ * tile that fits E, and E itself for elements some of whose tiles need more.  Where the tile
+ * path does not apply, the general kernel computes every element as tio_resample does.
+ */
+int tio_resample_tiered(const void* src, void* dst, int dtype,
+                        int B, int C, int I, int J, int K,
+                        int OI, int OJ, int OK,
+                        const float* mat, const float* cp, const uint8_t* flags,
+                        int ni, int nj, int nk,
+                        const float* spacing_in, const float* spacing_out,
+                        int affine_first, int mode, const float* fill, int box_hint,
+                        const int* elems, const int* runs, int n_runs,
+                        void* workspace, size_t workspace_bytes, void* stream);
 
 /*
  * The materialised form of label_interpolation="label", for the combinations the fused mode

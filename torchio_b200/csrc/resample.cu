@@ -154,17 +154,18 @@ __global__ void __launch_bounds__(256) min_kernel(const float* __restrict__ src,
 }
 
 int launch_resample_tile(const ResampleArgs& a, int dtype, int mode, bool exact_coords, int box_hint,
-                         void* workspace, size_t workspace_bytes, cudaStream_t st);
+                         const int* runs, int n_runs, void* workspace, size_t workspace_bytes, cudaStream_t st);
 size_t resample_tile_workspace_bytes(int B, int OI, int OJ, int OK);
 
 }  // namespace tio
 
-extern "C" int tio_resample(const void* src, void* dst, int dtype, int B, int C, int I, int J,
-                            int K, int OI, int OJ, int OK, const float* mat, const float* cp,
-                            const uint8_t* flags, int ni, int nj, int nk,
-                            const float* spacing_in, const float* spacing_out,
-                            int affine_first, int mode, const float* fill, int box_hint,
-                            void* workspace, size_t workspace_bytes, void* stream) {
+namespace {
+
+int resample(const void* src, void* dst, int dtype, int B, int C, int I, int J, int K, int OI, int OJ, int OK,
+             const float* mat, const float* cp, const uint8_t* flags, int ni, int nj, int nk,
+             const float* spacing_in, const float* spacing_out, int affine_first, int mode, const float* fill,
+             int box_hint, const int* elems, const int* runs, int n_runs, void* workspace, size_t workspace_bytes,
+             void* stream) {
   using namespace tio;
   TIO_CHECK_ARG(src && dst && mat, "tio_resample: null src/dst/mat");
   TIO_CHECK_ARG(src != dst, "tio_resample: src and dst must not alias");
@@ -180,7 +181,7 @@ extern "C" int tio_resample(const void* src, void* dst, int dtype, int B, int C,
   TIO_CHECK_ARG((int64_t)B * ((OI + TI - 1) / TI) <= 65535 && (OJ + TJ - 1) / TJ <= 65535,
                 "tio_resample: grid too large (B*ceil(OI/16) and ceil(OJ/4) must be <= 65535)");
   ResampleArgs a;
-  a.src = src; a.dst = dst; a.mat = mat; a.cp = cp; a.flags = flags; a.fill = fill;
+  a.src = src; a.dst = dst; a.mat = mat; a.cp = cp; a.flags = flags; a.fill = fill; a.elems = elems;
   a.B = B; a.C = C; a.I = I; a.J = J; a.K = K; a.OI = OI; a.OJ = OJ; a.OK = OK;
   a.ni = ni; a.nj = nj; a.nk = nk;
   auto scale = [](int n_in, int n_out) {
@@ -198,7 +199,8 @@ extern "C" int tio_resample(const void* src, void* dst, int dtype, int B, int C,
   a.cp_in_smem = cp && ((size_t)ni * nj * nk * 12 <= 96 * 1024);
   cudaStream_t st = (cudaStream_t)stream;
   if (box_hint >= 0) {  // fp32 trilinear and 1/2/4-byte nearest take the TMA tile path when it applies
-    const int rc = launch_resample_tile(a, dtype, mode, exact_coords, box_hint, workspace, workspace_bytes, st);
+    const int rc = launch_resample_tile(a, dtype, mode, exact_coords, box_hint, runs, n_runs, workspace,
+                                        workspace_bytes, st);
     if (rc == 0) {
       TIO_CHECK_LAUNCH();
       return 0;
@@ -216,6 +218,45 @@ extern "C" int tio_resample(const void* src, void* dst, int dtype, int B, int C,
   }
   TIO_CHECK_LAUNCH();
   return 0;
+}
+
+}  // namespace
+
+extern "C" int tio_resample(const void* src, void* dst, int dtype, int B, int C, int I, int J,
+                            int K, int OI, int OJ, int OK, const float* mat, const float* cp,
+                            const uint8_t* flags, int ni, int nj, int nk,
+                            const float* spacing_in, const float* spacing_out,
+                            int affine_first, int mode, const float* fill, int box_hint,
+                            void* workspace, size_t workspace_bytes, void* stream) {
+  return resample(src, dst, dtype, B, C, I, J, K, OI, OJ, OK, mat, cp, flags, ni, nj, nk, spacing_in, spacing_out,
+                  affine_first, mode, fill, box_hint, nullptr, nullptr, 0, workspace, workspace_bytes, stream);
+}
+
+extern "C" int tio_resample_tiered(const void* src, void* dst, int dtype, int B, int C, int I, int J,
+                                   int K, int OI, int OJ, int OK, const float* mat, const float* cp,
+                                   const uint8_t* flags, int ni, int nj, int nk,
+                                   const float* spacing_in, const float* spacing_out,
+                                   int affine_first, int mode, const float* fill, int box_hint,
+                                   const int* elems, const int* runs, int n_runs,
+                                   void* workspace, size_t workspace_bytes, void* stream) {
+  using namespace tio;
+  TIO_CHECK_ARG(elems && runs && n_runs >= 1 && n_runs <= 5, "tio_resample_tiered: null elems/runs or n_runs %d",
+                n_runs);
+  TIO_CHECK_ARG(dtype == TIO_F32 && mode == TIO_LINEAR && box_hint >= 0 && workspace,
+                "tio_resample_tiered: needs an fp32 image, TIO_LINEAR without TIO_EXACT_COORDS, box_hint >= 0 and"
+                " a workspace");
+  int total = 0, last = 0;
+  for (int r = 0; r < n_runs; ++r) {
+    const int count = runs[2 * r], edge = runs[2 * r + 1];
+    TIO_CHECK_ARG(count > 0 && edge > last && (edge == 20 || edge == 22 || edge == 24 || edge == 28 || edge == 32),
+                  "tio_resample_tiered: run %d: %d elements at edge %d (edges 20/22/24/28/32, ascending)", r, count,
+                  edge);
+    total += count;
+    last = edge;
+  }
+  TIO_CHECK_ARG(total == B, "tio_resample_tiered: the runs hold %d elements, the batch %d", total, B);
+  return resample(src, dst, dtype, B, C, I, J, K, OI, OJ, OK, mat, cp, flags, ni, nj, nk, spacing_in, spacing_out,
+                  affine_first, mode, fill, box_hint, elems, runs, n_runs, workspace, workspace_bytes, stream);
 }
 
 extern "C" size_t tio_resample_workspace_bytes(int B, int OI, int OJ, int OK) {

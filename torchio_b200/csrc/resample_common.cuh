@@ -33,6 +33,9 @@ struct ResampleArgs {
   const float* cp;       // [B][ni][nj][nk][3] or null
   const uint8_t* flags;  // [B] or null
   const float* fill;     // [C] or null
+  // TMA tile launches: batch element of each of the launch's B slots (device), or null = slot b
+  // is element b.  A tiered call runs one launch per box edge, each over its own elements.
+  const int* elems;
   int B, C, I, J, K, OI, OJ, OK;
   int ni, nj, nk;
   float sc_i, sc_j, sc_k;        // (n-1)/(O-1) upsample scales (fp32)

@@ -221,8 +221,9 @@ resample_fast_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_cons
 
   const int tid = threadIdx.x;
   const int tiles_i = ta.tiles_i;
-  const int b = tiles_i == 1 ? (int)blockIdx.z : (int)__umulhi(blockIdx.z, ta.inv_tiles_i);
-  const int ti = blockIdx.z - b * tiles_i;
+  const int slot = tiles_i == 1 ? (int)blockIdx.z : (int)__umulhi(blockIdx.z, ta.inv_tiles_i);
+  const int ti = blockIdx.z - slot * tiles_i;
+  const int b = a.elems ? __ldg(a.elems + slot) : slot;
   const int i0 = ti * XT, j0 = blockIdx.y * XT, k0 = blockIdx.x * XT;
   const unsigned tile_id = (blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
   const int4 rec = __ldg(records + tile_id);

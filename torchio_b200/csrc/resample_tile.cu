@@ -643,7 +643,7 @@ size_t resample_tile_workspace_bytes(int B, int OI, int OJ, int OK) {
 }
 
 int launch_resample_tile(const ResampleArgs& a, int dtype, int mode, bool exact_coords, int box_hint,
-                         void* workspace, size_t workspace_bytes, cudaStream_t st) {
+                         const int* runs, int n_runs, void* workspace, size_t workspace_bytes, cudaStream_t st) {
   // fp32 trilinear, or nearest for the 1/2/4-byte label types
   int esize = 0;
   if (mode == TIO_LINEAR) esize = dtype == TIO_F32 ? 4 : 0;
@@ -661,30 +661,28 @@ int launch_resample_tile(const ResampleArgs& a, int dtype, int mode, bool exact_
   const int tiles_i = (a.OI + XT - 1) / XT;
   if ((int64_t)a.B * tiles_i > 65535 || (a.OJ + XT - 1) / XT > 65535) return 1;
 
-  CUtensorMap tm;
   const cuuint64_t gdim[4] = {(cuuint64_t)a.K, (cuuint64_t)a.J, (cuuint64_t)a.I, (cuuint64_t)a.B * a.C};
   const cuuint64_t gstride[3] = {(cuuint64_t)a.K * esize, (cuuint64_t)a.J * a.K * esize,
                                  (cuuint64_t)a.I * a.J * a.K * esize};
-  const int bk = box_k_extent(box, esize);
-  const cuuint32_t bdim[4] = {(cuuint32_t)bk, (cuuint32_t)box, (cuuint32_t)box, 1};
   const cuuint32_t estr[4] = {1, 1, 1, 1};
   const CUtensorMapDataType ttype = mode == TIO_LINEAR ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
                                     : esize == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8
                                     : esize == 2 ? CU_TENSOR_MAP_DATA_TYPE_UINT16
                                                  : CU_TENSOR_MAP_DATA_TYPE_INT32;
-  CUresult rc = encode(&tm, ttype, 4, const_cast<void*>(a.src), gdim, gstride,
-                       bdim, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-                       CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (rc != CUDA_SUCCESS) return 1;
+  // tensor map of a box x box x box_k_extent(box) box
+  auto encode_box = [&](CUtensorMap* tm, int edge) {
+    const cuuint32_t bdim[4] = {(cuuint32_t)box_k_extent(edge, esize), (cuuint32_t)edge, (cuuint32_t)edge, 1};
+    return encode(tm, ttype, 4, const_cast<void*>(a.src), gdim, gstride, bdim, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                  CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+  };
 
   TileArgs ta;
-  const int dims[3] = {a.I, a.J, a.K};
   bool fast = true;
   for (int t = 0; t < 3; ++t) {
     ta.hd[t] = a.nm1[t] * 0.5f;
     ta.rcp[t] = (float)(1.0 / (double)ta.hd[t]);
     ta.hs[t] = a.sm1[t] * 0.5f;
-    (void)dims;
     fast = fast && fastdiv_admitted(ta.hd[t], st);
   }
   ta.n_in = (long long)a.I * a.J * a.K;
@@ -699,51 +697,58 @@ int launch_resample_tile(const ResampleArgs& a, int dtype, int mode, bool exact_
     ta.rsp_out[t] = (float)(1.0 / (double)a.sp_out[t]);
   }
 
-  dim3 grid((a.OK + XT - 1) / XT, (a.OJ + XT - 1) / XT, (unsigned)(a.B * tiles_i));
-  const int64_t n_tiles = (int64_t)grid.x * grid.y * grid.z;
+  const int64_t tiles_per_elem = (int64_t)tiles_i * ((a.OJ + XT - 1) / XT) * ((a.OK + XT - 1) / XT);
+  const int64_t n_tiles = (int64_t)a.B * tiles_per_elem;
   if (n_tiles >= (1ll << 31)) return 1;
   // per-tile records live in caller-provided workspace: no allocation, no state kept
   if (!workspace || workspace_bytes < (size_t)n_tiles * sizeof(int4) || ((uintptr_t)workspace & 15)) return 1;
-  int4* records = (int4*)workspace;
-  const unsigned bounds_blocks = (unsigned)((n_tiles + 127) / 128);
   if (mode != TIO_LINEAR && !fast) return 1;
   // elastic launches of the fast kernel: most tiles need far less than the launch's box (the
   // displacement is smooth, its borders are locked) and load a small box instead
-  const bool dual = !exact_coords && mode == TIO_LINEAR && a.cp && box > kSmallBox;
-  const int box_s = dual ? kSmallBox : 0, bk_s = dual ? box_k_extent(kSmallBox, 4) : 0;
-  CUtensorMap tm_small = tm;
-  if (dual) {
-    const cuuint32_t bdim_s[4] = {(cuuint32_t)bk_s, (cuuint32_t)box_s, (cuuint32_t)box_s, 1};
-    if (encode(&tm_small, ttype, 4, const_cast<void*>(a.src), gdim, gstride, bdim_s, estr,
-               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return 1;
+  const bool dual = !exact_coords && mode == TIO_LINEAR && a.cp;  // every edge is > kSmallBox
+  CUtensorMap tm_small;
+  if (dual && !encode_box(&tm_small, kSmallBox)) return 1;
+
+  // one launch pair (bounds pre-pass, tile kernel) per run of slots sharing a box edge: the
+  // caller's runs for a tiered call (a.elems set), else all B elements at `box`
+  const int whole[2] = {a.B, box};
+  if (!a.elems) { runs = whole; n_runs = 1; }
+  CUtensorMap tms[5];
+  for (int r = 0; r < n_runs; ++r)
+    if (!encode_box(&tms[r], runs[2 * r + 1])) return 1;
+  int offset = 0;
+  for (int r = 0; r < n_runs; ++r) {
+    const int count = runs[2 * r], edge = runs[2 * r + 1];
+    const CUtensorMap& tm = tms[r];
+    ResampleArgs ar = a;
+    ar.B = count;
+    ar.elems = a.elems ? a.elems + offset : nullptr;
+    int4* records = (int4*)workspace + offset * tiles_per_elem;
+    offset += count;
+    const dim3 grid((a.OK + XT - 1) / XT, (a.OJ + XT - 1) / XT, (unsigned)(count * tiles_i));
+    const int bk = box_k_extent(edge, esize);
+    const int box_s = dual ? kSmallBox : 0, bk_s = dual ? box_k_extent(kSmallBox, 4) : 0;
+    const unsigned bounds_blocks = (unsigned)((count * tiles_per_elem + 127) / 128);
+    if (ar.cp) tile_bounds_kernel<true><<<bounds_blocks, 128, 0, st>>>(ar, edge, kalign, bk, box_s, bk_s, records);
+    else tile_bounds_kernel<false><<<bounds_blocks, 128, 0, st>>>(ar, edge, kalign, bk, box_s, bk_s, records);
+    launched();
+    const size_t smem = ((size_t)edge * edge * bk * esize + 15) / 16 * 16 + kAuxFloats * sizeof(float);
+    if (mode == TIO_LABEL_PV) {
+      if (dtype == TIO_U8) launch_label_pv<uint8_t>(edge, tm, ar, ta, grid, smem, records, st);
+      else if (dtype == TIO_I16) launch_label_pv<int16_t>(edge, tm, ar, ta, grid, smem, records, st);
+      else launch_label_pv<int32_t>(edge, tm, ar, ta, grid, smem, records, st);
+    } else if (mode == TIO_NEAREST) {
+      if (dtype == TIO_U8) launch_nearest<uint8_t>(edge, tm, ar, ta, grid, smem, records, st);
+      else if (dtype == TIO_I16) launch_nearest<int16_t>(edge, tm, ar, ta, grid, smem, records, st);
+      else launch_nearest<int32_t>(edge, tm, ar, ta, grid, smem, records, st);
+    } else if (!exact_coords) {  // fp32 images: one-fma coordinates where no tap can leave the volume
+      launch_resample_fast(edge, tm, dual ? tm_small : tm, ar, ta, grid, smem, records, st);
+    } else if (edge == 20) launch_box<20>(tm, ar, ta, grid, smem, fast, records, st);
+    else if (edge == 22) launch_box<22>(tm, ar, ta, grid, smem, fast, records, st);
+    else if (edge == 24) launch_box<24>(tm, ar, ta, grid, smem, fast, records, st);
+    else if (edge == 28) launch_box<28>(tm, ar, ta, grid, smem, fast, records, st);
+    else launch_box<32>(tm, ar, ta, grid, smem, fast, records, st);
   }
-  if (a.cp) tile_bounds_kernel<true><<<bounds_blocks, 128, 0, st>>>(a, box, kalign, bk, box_s, bk_s, records);
-  else tile_bounds_kernel<false><<<bounds_blocks, 128, 0, st>>>(a, box, kalign, bk, box_s, bk_s, records);
-  launched();
-  const size_t smem = ((size_t)box * box * bk * esize + 15) / 16 * 16 + kAuxFloats * sizeof(float);
-  if (mode == TIO_LABEL_PV) {
-    if (dtype == TIO_U8) launch_label_pv<uint8_t>(box, tm, a, ta, grid, smem, records, st);
-    else if (dtype == TIO_I16) launch_label_pv<int16_t>(box, tm, a, ta, grid, smem, records, st);
-    else launch_label_pv<int32_t>(box, tm, a, ta, grid, smem, records, st);
-    return 0;
-  }
-  if (mode == TIO_NEAREST) {
-    if (dtype == TIO_U8) launch_nearest<uint8_t>(box, tm, a, ta, grid, smem, records, st);
-    else if (dtype == TIO_I16) launch_nearest<int16_t>(box, tm, a, ta, grid, smem, records, st);
-    else launch_nearest<int32_t>(box, tm, a, ta, grid, smem, records, st);
-    return 0;
-  }
-  if (!exact_coords) {  // fp32 images: one-fma coordinates where no tap can leave the volume
-    launch_resample_fast(box, tm, tm_small, a, ta, grid, smem, records, st);
-    return 0;
-  }
-  if (box == 20) launch_box<20>(tm, a, ta, grid, smem, fast, records, st);
-  else if (box == 22) launch_box<22>(tm, a, ta, grid, smem, fast, records, st);
-  else if (box == 24) launch_box<24>(tm, a, ta, grid, smem, fast, records, st);
-  else if (box == 28) launch_box<28>(tm, a, ta, grid, smem, fast, records, st);
-  else launch_box<32>(tm, a, ta, grid, smem, fast, records, st);
   return 0;
 }
 

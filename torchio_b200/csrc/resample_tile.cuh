@@ -134,8 +134,9 @@ tile_bounds_kernel(const ResampleArgs a, const int box, const int kalign, const 
   const int64_t tile = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (tile >= n_tiles) return;
   const unsigned per_b = (unsigned)(tiles_i * tiles_j * tiles_k);
-  const int b = (int)(tile / per_b);
-  unsigned rest = (unsigned)(tile - (int64_t)b * per_b);
+  const int slot = (int)(tile / per_b);
+  const int b = a.elems ? a.elems[slot] : slot;
+  unsigned rest = (unsigned)(tile - (int64_t)slot * per_b);
   const int tk = (int)(rest % (unsigned)tiles_k);
   rest /= (unsigned)tiles_k;
   const int tj = (int)(rest % (unsigned)tiles_j), ti = (int)(rest / (unsigned)tiles_j);

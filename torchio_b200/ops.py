@@ -189,6 +189,7 @@ def resample(
     src: Tensor, mat: Tensor, cp: Tensor | None, flags: Tensor | None,
     spacing_in, spacing_out, *, affine_first: bool, mode: int,
     fill: Tensor | None, out_shape=None, box_hint: int = 0, exact_coords: bool | None = None,
+    tiers=None,
 ) -> Tensor:
     """K1.  Replaces _build_sampling_grid + _sample_batch[_per_sample]
     (spatial/spatial.py:1504-1579,1651-1857).
@@ -202,8 +203,13 @@ def resample(
     trilinear voxels whose taps all lie inside the volume use one fma per axis, which differs
     from the reference by its own coordinate noise (<= ~2e-5 voxel); label maps, padding and
     fill decisions are exact either way.
+
+    tiers: ``(elems, runs)`` for a box edge per element (`tio_resample_tiered`): ``elems`` an
+    int32 (B,) cuda permutation of the batch, ``runs`` ``[(count, edge), ...]`` over it in
+    ascending edges.  fp32 trilinear without exact coordinates only; same output as without.
     """
     src = _batch(src, "resample", dtypes=DTYPE_CODES)
+    exact = _exact_default if exact_coords is None else exact_coords
     b, c, i, j, k = src.shape
     oi, oj, ok = (i, j, k) if out_shape is None else out_shape
     dst = torch.empty((b, c, oi, oj, ok), dtype=src.dtype, device=src.device)
@@ -218,13 +224,19 @@ def resample(
     if box_hint >= 0 and tiled:
         ws_bytes = _native.lib().tio_resample_workspace_bytes(b, oi, oj, ok)
         workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=src.device)
-    _launch(
-        "tio_resample", src.device, _ptr(src), _ptr(dst), DTYPE_CODES[src.dtype],
-        b, c, i, j, k, oi, oj, ok, _ptr(mat), _ptr(cp), _ptr(flags), ni, nj, nk,
-        sp_in.ctypes.data, sp_out.ctypes.data, int(bool(affine_first)),
-        int(mode) | (EXACT_COORDS if (_exact_default if exact_coords is None else exact_coords) else 0),
-        _ptr(fill), int(box_hint), _ptr(workspace), ws_bytes,
-    )
+    args = (_ptr(src), _ptr(dst), DTYPE_CODES[src.dtype],
+            b, c, i, j, k, oi, oj, ok, _ptr(mat), _ptr(cp), _ptr(flags), ni, nj, nk,
+            sp_in.ctypes.data, sp_out.ctypes.data, int(bool(affine_first)),
+            int(mode) | (EXACT_COORDS if exact else 0), _ptr(fill), int(box_hint))
+    if tiers is None:
+        _launch("tio_resample", src.device, *args, _ptr(workspace), ws_bytes)
+        return dst
+    elems, runs = tiers
+    if elems.dtype != torch.int32 or elems.shape != (b,) or not elems.is_cuda:
+        raise ValueError(f"resample: tiers needs an int32 ({b},) cuda element list")
+    runs = np.asarray(runs, dtype=np.int32).reshape(-1, 2)
+    _launch("tio_resample_tiered", src.device, *args, _ptr(elems), runs.ctypes.data, len(runs),
+            _ptr(workspace), ws_bytes)
     return dst
 
 

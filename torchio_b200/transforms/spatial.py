@@ -846,8 +846,10 @@ def _apply_spatial(batch, names, target_space, geometry, *, affine_first, image_
     if info is None:  # streamed batches: checked once on the whole batch (Spatial.plan_checks)
         _folding_warning(cps, max_displacements, out_shape, a_out)
     device = first.data.device
-    mat_d, cp_d, flags_d = ops.upload(device, packed.mat, packed.cp, packed.flags)
     box_hint = _box_hint(packed, a_in.spacing, a_out.spacing, out_shape)
+    order, runs = _box_tiers(packed, box_hint, out_shape)
+    mat_d, cp_d, flags_d, order_d = ops.upload(device, packed.mat, packed.cp, packed.flags, order)
+    tiers = None if order is None else (order_d, runs)
     target_shape = None if target_space is None else out_shape
 
     def spline(tensor, order, in_place, source=None):
@@ -893,11 +895,12 @@ def _apply_spatial(batch, names, target_space, geometry, *, affine_first, image_
             fill = info.cache[("fill", info.step, name)]
         if antialias and not is_label:  # after the fill value (spatial.py:1249-1257): blur what is downsampled
             native = _antialias(native, a_in, a_out)
+        mode = ops.NEAREST if interp == "nearest" else ops.LINEAR
+        tiered = mode == ops.LINEAR and native.dtype == torch.float32 and not ops.exact_coords_default()
         out = ops.resample(
             native, mat_d, cp_d, flags_d, a_in.spacing, a_out.spacing,
-            affine_first=affine_first, mode=ops.NEAREST if interp == "nearest" else ops.LINEAR,
-            fill=fill, out_shape=target_shape,
-            box_hint=box_hint,
+            affine_first=affine_first, mode=mode, fill=fill, out_shape=target_shape,
+            box_hint=box_hint, tiers=tiers if tiered else None,
         )
         ib.data = out if out.dtype == data.dtype else out.to(data.dtype)
         ib.affines[:] = [
@@ -931,6 +934,52 @@ def _box_hint(packed, sp_in, sp_out, out_shape) -> int:
         if worst <= edge:
             return edge
     return 32
+
+
+_BOX_EDGES = (20, 22, 24, 28, 32)
+
+
+def _box_tiers(packed, cap: int, out_shape):
+    """Box edge per element for the affine-only fp32 trilinear launches: (elements ordered by
+    edge as int32, [(count, edge), ...] ascending), or (None, None) when every element needs the
+    launch's own box ``cap`` (or the call has a control grid: elastic launches keep one box).
+    A smaller box leaves more shared memory and registers per SM: boxes of 20 and 22 run four
+    CTAs per SM, 24 three."""
+    if packed.cp is not None:
+        return None, None
+    edges = _affine_box_edges(packed.mat, cap, out_shape)
+    if (edges == cap).all():
+        return None, None
+    order = np.argsort(edges, kind="stable").astype(np.int32)
+    values, counts = np.unique(edges, return_counts=True)
+    return order, [(int(n), int(e)) for e, n in zip(values, counts)]
+
+
+def _affine_box_edges(mat, cap: int, out_shape) -> np.ndarray:
+    """Per element of an affine-only launch: the smallest box edge (of `_BOX_EDGES`, at most
+    ``cap``, the launch's own box) whose edge x edge x box_k_extent(edge) box holds the pre-image
+    of every 16^3 output tile, as `tile_bounds_kernel` measures it; ``cap`` where none does.
+
+    The pre-pass takes, per input axis, q in [qlo, qhi] with qhi - qlo <= 15 * sum_b |M_ab| widened
+    by its margin 0.02 + 1e-5 |q| on each side, then lo = floor(qlo), hi = floor(qhi) + 1, so a tile
+    needs at most floor(width) + 3 planes, and K three more for rounding lo down to 16 bytes.
+    The 1e-3 covers the pre-pass's fp32 rounding.  Since no tile needs more than its element's
+    edge, and a tile that does not fit ``cap`` is never moved below it, every tile takes the same
+    path (staged box or fallback) as in a launch of ``cap`` for all."""
+    m = np.asarray(mat, dtype=np.float64).reshape(-1, 3, 4)
+    lin = np.abs(m[:, :, :3])
+    span = np.maximum(np.asarray(out_shape, dtype=np.float64) - 1.0, 0.0)
+    q_max = np.abs(m[:, :, 3]) + lin @ span  # bound of |q| over the whole output
+    width = lin.sum(axis=2) * 15.0 + 2.0 * (0.02 + 1e-5 * q_max) + 1e-3
+    with np.errstate(invalid="ignore"):
+        need = np.floor(width) + 3.0
+        need[:, 2] += 3.0
+        need[~np.isfinite(need)] = np.inf
+        edges = np.full(len(m), cap, dtype=np.int32)
+        for edge in reversed([e for e in _BOX_EDGES if e < cap]):
+            fits = (need[:, 0] <= edge) & (need[:, 1] <= edge) & (need[:, 2] <= (edge + 7) // 4 * 4)
+            edges[fits] = edge
+    return edges
 
 
 class Resample(Spatial):
