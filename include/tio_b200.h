@@ -171,6 +171,27 @@ int tio_resample_tiered(const void* src, void* dst, int dtype,
                         int affine_first, int mode, const float* fill, int box_hint,
                         const int* elems, const int* runs, int n_runs,
                         void* workspace, size_t workspace_bytes, void* stream);
+/*
+ * K1ᵀ — the adjoint of tio_resample with respect to src, for fp32 gradients: grad_in (B, C, I, J, K)
+ * = K1ᵀ grad_out (B, C, OI, OJ, OK), with the geometry arguments of the forward call (mode
+ * TIO_NEAREST or TIO_LINEAR, TIO_EXACT_COORDS accepted).  Replaces the backward of the reference's
+ * F.grid_sample / torch.where (spatial.py:1651-1731, 1764-1857): each output voxel sends g * w to each
+ * in-bounds trilinear tap (nearest: g to the rounded voxel), a voxel the forward filled (fill given
+ * and mask <= 0.5) sends nothing, and TIO_FLAG_PASSTHROUGH elements copy g, which needs
+ * (OI, OJ, OK) == (I, J, K) as in tio_resample (flags live on the device: the library cannot check).
+ * Coordinates, weights and fill decisions follow the reference's fp32 chain in both coordinate
+ * modes.  grad_in is zeroed (cudaMemsetAsync), then one bounds pre-pass and one tile launch add into
+ * it with atomics: the result is not deterministic.  workspace: tio_resample_workspace_bytes(B, OI,
+ * OJ, OK) bytes, 16-byte aligned, required.  box_hint > 24 selects 32^3 boxes, else 24^3.
+ */
+int tio_resample_backward(const float* grad_out, float* grad_in,
+                          int B, int C, int I, int J, int K,
+                          int OI, int OJ, int OK,
+                          const float* mat, const float* cp, const uint8_t* flags,
+                          int ni, int nj, int nk,
+                          const float* spacing_in, const float* spacing_out,
+                          int affine_first, int mode, const float* fill, int box_hint,
+                          void* workspace, size_t workspace_bytes, void* stream);
 
 /*
  * The materialised form of label_interpolation="label", for the combinations the fused mode

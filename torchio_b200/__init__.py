@@ -14,7 +14,7 @@ of ``include/tio_b200.h``; see DESIGN.md and INTEGRATION.md.
 
 from .data import (AffineMatrix, Image, ImagesBatch, LabelMap, ScalarImage, StudiesBatch,
                    Subject, SubjectsBatch)
-from .ops import exact_coords_default, set_exact_coords
+from .ops import differentiable_default, exact_coords_default, set_differentiable, set_exact_coords
 from .params import Choice
 from .patches import (GridSampler, ImagesLoader, LabelSampler, PatchAggregator, PatchLocation, PatchSampler, Queue,
                       StudiesLoader, SubjectsLoader, UniformSampler, WeightedSampler, collate_images, collate_studies,
@@ -35,6 +35,6 @@ __all__ = [
     "Reorient", "Resample", "RescaleIntensity", "Resize", "ScalarImage", "SequentialLabels", "Spatial",
     "SpatialTransform", "Spike", "Standardize", "StudiesBatch", "StudiesLoader", "Subject", "SubjectsBatch",
     "SubjectsLoader", "Swap", "ToReferenceSpace", "Transform", "Transpose", "UniformSampler", "WeightedSampler", "ZNormalization", "apply_inverse_transform", "collate_images",
-    "collate_studies", "collate_subjects", "exact_coords_default", "execution_device", "get_inverse_transform",
-    "set_exact_coords", "set_execution_device",
+    "collate_studies", "collate_subjects", "differentiable_default", "exact_coords_default", "execution_device", "get_inverse_transform",
+    "set_differentiable", "set_exact_coords", "set_execution_device",
 ]

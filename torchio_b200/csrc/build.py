@@ -17,7 +17,7 @@ from pathlib import Path
 
 HERE = Path(__file__).resolve().parent
 ROOT = HERE.parent.parent
-SOURCES = ["error.cu", "resample.cu", "resample_tile.cu", "resample_fast.cu", "upload.cu", "fused_intensity.cu",
+SOURCES = ["error.cu", "resample.cu", "resample_tile.cu", "resample_fast.cu", "resample_backward.cu", "upload.cu", "fused_intensity.cu",
            "mt19937_jump.cpp", "mt19937.cu", "patches.cu", "stats.cu", "labels.cu", "labels_to_image.cu",
            "label_maps.cu", "interpolate.cu", "clamp_mask_swap.cu", "components.cu", "permute.cu", "spike.cu",
            "ghosting.cu", "motion.cu", "aggregate.cu", "bspline.cu", "pca.cu"]

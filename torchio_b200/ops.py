@@ -185,6 +185,26 @@ def exact_coords_default() -> bool:
     return _exact_default
 
 
+_differentiable = False
+
+
+def set_differentiable(enabled: bool) -> bool:
+    """Process-wide switch of the transforms' differentiable path; returns the previous value.
+
+    Off (the default), a transform refuses an image that requires grad.  On, a transform of the
+    differentiable set (see `torchio_b200.autograd`) records a graph node when
+    ``torch.is_grad_enabled()`` and an image it modifies requires grad, and any other transform
+    that would modify such an image raises NotImplementedError naming itself.  The ``ops``
+    functions themselves stay forward-only either way."""
+    global _differentiable
+    previous, _differentiable = _differentiable, bool(enabled)
+    return previous
+
+
+def differentiable_default() -> bool:
+    return _differentiable
+
+
 def resample(
     src: Tensor, mat: Tensor, cp: Tensor | None, flags: Tensor | None,
     spacing_in, spacing_out, *, affine_first: bool, mode: int,
@@ -238,6 +258,32 @@ def resample(
     _launch("tio_resample_tiered", src.device, *args, _ptr(elems), runs.ctypes.data, len(runs),
             _ptr(workspace), ws_bytes)
     return dst
+
+
+def resample_backward(
+    grad_out: Tensor, in_shape, mat: Tensor, cp: Tensor | None, flags: Tensor | None,
+    spacing_in, spacing_out, *, affine_first: bool, mode: int, fill: Tensor | None, box_hint: int = 0,
+) -> Tensor:
+    """K1ᵀ (`tio_resample_backward`): the fp32 (B, C, *in_shape) gradient of `resample`'s input for
+    the fp32 (B, C, OI, OJ, OK) gradient ``grad_out`` of its output, same geometry arguments, modes
+    NEAREST and LINEAR.  Not deterministic: the taps are added with atomics."""
+    grad_out = _batch(grad_out, "resample_backward", dtypes=(torch.float32,))
+    b, c, oi, oj, ok = grad_out.shape
+    i, j, k = (int(v) for v in in_shape)
+    if mode not in (NEAREST, LINEAR):
+        raise ValueError(f"resample_backward: mode {mode} has no adjoint kernel")
+    grad_in = torch.empty((b, c, i, j, k), dtype=torch.float32, device=grad_out.device)
+    ni = nj = nk = 0
+    if cp is not None:
+        ni, nj, nk = cp.shape[1:4]
+    sp_in = np.asarray(spacing_in, dtype=np.float32)
+    sp_out = np.asarray(spacing_out, dtype=np.float32)
+    ws_bytes = _native.lib().tio_resample_workspace_bytes(b, oi, oj, ok)
+    workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=grad_out.device)
+    _launch("tio_resample_backward", grad_out.device, _ptr(grad_out), _ptr(grad_in), b, c, i, j, k, oi, oj, ok,
+            _ptr(mat), _ptr(cp), _ptr(flags), ni, nj, nk, sp_in.ctypes.data, sp_out.ctypes.data,
+            int(bool(affine_first)), int(mode), _ptr(fill), int(box_hint), _ptr(workspace), ws_bytes)
+    return grad_in
 
 
 def bspline_prefilter(src: Tensor, order: int, flags: Tensor | None = None, *, in_place: bool = False) -> Tensor:

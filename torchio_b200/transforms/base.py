@@ -29,6 +29,7 @@ import numpy as np
 import torch
 from torch import Tensor, nn
 
+from .. import autograd, ops
 from ..data import Image, ImagesBatch, ScalarImage, Subject, SubjectsBatch
 from ..params import _ParameterRange
 
@@ -116,6 +117,19 @@ def staged_source_device(name: str, data: Tensor) -> torch.device:
     return data.device
 
 
+def refuse_host_grad(batch: SubjectsBatch) -> None:
+    """With `set_differentiable(True)`, refuse a host-resident image that requires grad: a graph
+    is recorded for CUDA tensors only, never across the staging copies."""
+    if not ops.differentiable_default():
+        return
+    for name, ib in batch.images.items():
+        t = ib.data
+        if t.requires_grad and not t.is_cuda:
+            raise NotImplementedError(
+                f'image "{name}" requires grad and lives on {t.device}: gradients are computed for'
+                " CUDA tensors only; move the batch to the GPU first")
+
+
 class _Staging:
     """Move a CPU batch to the execution device and back, preserving pinning.  Images a transform
     adds during the call are brought back like the image they were derived from."""
@@ -125,6 +139,7 @@ class _Staging:
         self.origin: dict[str, tuple[torch.device, bool]] = {}
 
     def __enter__(self):
+        refuse_host_grad(self.batch)
         dev = None
         for name, ib in self.batch.images.items():
             t = ib.data
@@ -239,10 +254,22 @@ class Transform(nn.Module):
         # torch.rand(1) is drawn even when p == 1 (transform.py:227)
         if not self._per_instance_p_active(batch) and torch.rand(1).item() >= self.p:
             return batch
+        self._check_differentiable(batch)
         params = self.make_params(batch)
         batch = self.apply_transform(batch, params)
         self._record(batch, params)
         return batch
+
+    #: The transform has a differentiable path (`torchio_b200.autograd`).
+    differentiable = False
+
+    def _check_differentiable(self, batch: SubjectsBatch) -> None:
+        """With `set_differentiable(True)` and grad mode on, refuse to modify an image that
+        requires grad unless the transform has a differentiable path: never detach silently."""
+        if self.differentiable or not ops.differentiable_default() or not torch.is_grad_enabled():
+            return
+        if any(ib.data.requires_grad for ib in self._get_images(batch).values()):
+            autograd.refuse(type(self).__name__)
 
     def _record(self, batch: SubjectsBatch, params: dict[str, Any]) -> None:
         if _all_gated_out(params):

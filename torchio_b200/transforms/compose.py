@@ -17,8 +17,10 @@ import torch as _torch
 
 from ..data import ImagesBatch, SubjectsBatch
 from ..params import slice_params
-from .base import ChunkInfo, Transform, _Staging, _finish, chunk_scope, execution_device, wrap_input
+from .base import (ChunkInfo, Transform, _Staging, _finish, chunk_scope, execution_device, refuse_host_grad,
+                   wrap_input)
 from . import intensity as _int
+from .. import ops as _ops
 
 
 _stream_local = _threading.local()
@@ -52,7 +54,7 @@ class Compose(Transform):
             self.transforms = list(transforms)
 
     def forward(self, data: Any) -> Any:
-        return self.submit(data).result()
+        return self._submit(data, graph=True).result()
 
     def submit(self, data: Any) -> "Pending":
         """Issue the whole pipeline for ``data`` and return without waiting for the device.
@@ -67,9 +69,19 @@ class Compose(Transform):
         Until `result()` returns, the device is still reading the host tensors of ``data``: a
         loader that refills one staging buffer in place must not touch it before then (fresh
         tensors per batch, as `SubjectsLoader` / `DataLoader` produce, are fine)."""
+        return self._submit(data, graph=False)
+
+    def _submit(self, data: Any, graph: bool) -> "Pending":
+        """`submit`; ``graph``: a batch that requires grad may record a graph (`forward` only: a
+        ticket cannot hand back a graph node)."""
         if self.copy:
             data = _copy.deepcopy(data)
         batch, unwrap = wrap_input(data)
+        if not graph and _ops.differentiable_default() and any(
+                ib.data.requires_grad for ib in batch.images.values()):
+            raise NotImplementedError("Compose.submit / Compose.stream: inputs that require grad are not"
+                                      " supported; call the Compose itself")
+        refuse_host_grad(batch)  # before the streamed path, which does not stage through _Staging
         chunk = self._chunk_size(batch)
         if chunk:
             batch, done = self._forward_streamed(batch, chunk)
@@ -307,6 +319,8 @@ def _run_fused(group: list[Transform], batch):
     (gate draw, then make_params, in order — none of them reads voxel data),
     then apply all non-gated stages with one fused launch pair per image."""
     applied = _sample_group(group, batch)
+    for transform, _ in applied:
+        transform._check_differentiable(batch)
     if applied:
         _apply_group(applied, batch)
         for transform, params in applied:

@@ -31,7 +31,7 @@ import torch
 from torch import Tensor
 from torch.distributions import Distribution
 
-from .. import ops, tables
+from .. import autograd, ops, tables
 from ..data import AffineMatrix, Image, ImagesBatch, LabelMap, SubjectsBatch
 from ..params import Choice, LazyParams, _ParameterRange, to_range, uniform_from_unit
 from .base import SpatialTransform, chunk_info
@@ -374,6 +374,8 @@ def _antialias(data, a_in: AffineMatrix, a_out: AffineMatrix):
 class Spatial(SpatialTransform):
     """Resample + affine + elastic in one fused pass (spatial.py:158-369)."""
 
+    differentiable = True  # orders 0-1 without antialias: autograd.resample
+
     def __init__(self, *, target=None, scales=1.0, degrees=0.0, translation=0.0,
                  isotropic: bool = False, center: str = "image", control_points=None,
                  num_control_points=7, max_displacement=0.0, locked_borders: int = 2,
@@ -646,7 +648,7 @@ class Spatial(SpatialTransform):
             antialias=params.get("antialias", False),
             one_hot_label_interpolation=params.get("one_hot_label_interpolation", "linear"),
             default_pad_value=params["default_pad_value"],
-            default_pad_label=float(params["default_pad_label"]),
+            default_pad_label=float(params["default_pad_label"]), transform=type(self).__name__,
         )
         return batch
 
@@ -694,6 +696,8 @@ def _unpack_geometry(params):
 class _SpatialInverse(SpatialTransform):
     """Concrete inverse used by history replay (spatial.py:679-756)."""
 
+    differentiable = True
+
     def __init__(self, *, target, geometry, affine_first, image_interpolation,
                  label_interpolation, default_pad_value, default_pad_label,
                  one_hot_label_interpolation="linear", **kwargs: Any):
@@ -714,6 +718,7 @@ class _SpatialInverse(SpatialTransform):
             label_interpolation=self.label_interpolation, antialias=False,
             one_hot_label_interpolation=self.one_hot_label_interpolation,
             default_pad_value=self.default_pad_value, default_pad_label=self.default_pad_label,
+            transform=type(self).__name__,
         )
         return batch
 
@@ -815,7 +820,8 @@ def _resample_label_pv(data, resample, spline, *, antialias, a_in, a_out, one_ho
 
 def _apply_spatial(batch, names, target_space, geometry, *, affine_first, image_interpolation,
                    label_interpolation, antialias, default_pad_value, default_pad_label,
-                   one_hot_label_interpolation="linear", max_displacements=None) -> None:
+                   one_hot_label_interpolation="linear", max_displacements=None,
+                   transform: str = "Spatial") -> None:
     if not names:
         return
     mats, cps, per_instance = geometry
@@ -867,6 +873,16 @@ def _apply_spatial(batch, names, target_space, geometry, *, affine_first, image_
         is_label = issubclass(ib._image_class, LabelMap)
         interp = label_interpolation if is_label else image_interpolation
         data = ib.data
+        graph = autograd.records_graph(data)
+        if graph:
+            if is_label:
+                autograd.refuse(transform, f'label map "{name}"')
+            if interp == LABEL_INTERPOLATION or _ORDERS[interp] >= 2:
+                autograd.refuse(transform, f'interpolation "{interp}"')
+            if antialias:
+                autograd.refuse(transform, "antialias")
+        elif data.requires_grad and ops.differentiable_default():
+            data = data.detach()  # grad mode is off: no graph to record, the usual kernels run
         if is_label and interp == LABEL_INTERPOLATION:
             def run(tensor, mode, fill, exact):
                 return ops.resample(
@@ -889,16 +905,18 @@ def _apply_spatial(batch, names, target_space, geometry, *, affine_first, image_
             ib.data = out
             ib.affines[:] = [ib.affines[i] if i in keep_original else a_out.clone() for i in range(b)]
             continue
-        if info is None:
-            fill = _fill_tensor(native, is_label, default_pad_value, default_pad_label)
+        if info is None:  # fill statistics are constants of the graph (the reference takes .item())
+            fill = _fill_tensor(native.detach() if graph else native, is_label, default_pad_value,
+                                default_pad_label)
         else:  # streamed: derived from batch element 0 when the first slice came through
             fill = info.cache[("fill", info.step, name)]
         if antialias and not is_label:  # after the fill value (spatial.py:1249-1257): blur what is downsampled
             native = _antialias(native, a_in, a_out)
         mode = ops.NEAREST if interp == "nearest" else ops.LINEAR
         tiered = mode == ops.LINEAR and native.dtype == torch.float32 and not ops.exact_coords_default()
-        out = ops.resample(
-            native, mat_d, cp_d, flags_d, a_in.spacing, a_out.spacing,
+        resample = autograd.resample if graph else ops.resample
+        out = resample(
+            native, mat=mat_d, cp=cp_d, flags=flags_d, spacing_in=a_in.spacing, spacing_out=a_out.spacing,
             affine_first=affine_first, mode=mode, fill=fill, out_shape=target_shape,
             box_hint=box_hint, tiers=tiers if tiered else None,
         )
