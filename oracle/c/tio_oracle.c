@@ -123,6 +123,108 @@ static inline float affine_row(const float* m, float pi, float pj, float pk) {
   return acc;
 }
 
+/* Geometry of one orc_resample / orc_resample_adjoint call, shared by every voxel. */
+typedef struct {
+  int I, J, K, OI, OJ, OK, ni, nj, nk, affine_first, mode, has_fill;
+  const float *spacing_in, *spacing_out;
+  float nm1[3], sm1[3];
+} orc_geom;
+
+static orc_geom geom_of(int I, int J, int K, int OI, int OJ, int OK, int ni, int nj, int nk,
+                        const float* spacing_in, const float* spacing_out, int affine_first,
+                        int mode, int has_fill) {
+  orc_geom G;
+  G.I = I; G.J = J; G.K = K; G.OI = OI; G.OJ = OJ; G.OK = OK;
+  G.ni = ni; G.nj = nj; G.nk = nk;
+  G.spacing_in = spacing_in; G.spacing_out = spacing_out;
+  G.affine_first = affine_first; G.mode = mode; G.has_fill = has_fill;
+  /* max(size-1, 1) (spatial.py:1638-1640) */
+  G.nm1[0] = (float)(I - 1 > 1 ? I - 1 : 1);
+  G.nm1[1] = (float)(J - 1 > 1 ? J - 1 : 1);
+  G.nm1[2] = (float)(K - 1 > 1 ? K - 1 : 1);
+  /* ATen un-normalise multiplies by (size - 1) without the max() */
+  G.sm1[0] = (float)(I - 1); G.sm1[1] = (float)(J - 1); G.sm1[2] = (float)(K - 1);
+  return G;
+}
+
+/* What output voxel (oi, oj, ok) reads: its 8 trilinear corners (weight, in-bounds bit, offset
+ * in the input volume), whether the fill replaces it, and its nearest-mode voxel (-1: outside).
+ * The one per-voxel chain of orc_resample and orc_resample_adjoint, so the adjoint's weights and
+ * fill decisions are the forward's. */
+typedef struct {
+  float w8[8];
+  int inb[8];
+  int64_t off8[8];
+  int use_fill;
+  int64_t nn_off;
+} orc_voxel;
+
+static void resample_voxel(const orc_geom* G, const float* m, const float* g, int oi, int oj,
+                           int ok, orc_voxel* v) {
+  const int I = G->I, J = G->J, K = G->K;
+  const int dims[3] = {I, J, K};
+  float p[3] = {(float)oi, (float)oj, (float)ok};
+  float d[3] = {0.f, 0.f, 0.f};
+  if (g) { /* spatial.py:2171-2189 */
+    int i0, i1, j0, j1, k0, k1; float a0, a1, b0, b1, c0, c1;
+    lerp_setup(G->ni, G->OI, oi, &i0, &i1, &a0, &a1);
+    lerp_setup(G->nj, G->OJ, oj, &j0, &j1, &b0, &b1);
+    lerp_setup(G->nk, G->OK, ok, &k0, &k1, &c0, &c1);
+    for (int a = 0; a < 3; ++a)
+      d[a] = trilerp(g + a, G->nj, G->nk, 3, i0, i1, a0, a1, j0, j1, b0, b1, k0, k1, c0, c1);
+  }
+  float q[3];
+  if (!g) {
+    for (int a = 0; a < 3; ++a) q[a] = affine_row(m + 4 * a, p[0], p[1], p[2]);
+  } else if (G->affine_first) { /* spatial.py:1570-1573 */
+    for (int a = 0; a < 3; ++a)
+      q[a] = affine_row(m + 4 * a, p[0], p[1], p[2]) + fdiv(d[a], G->spacing_in[a]);
+  } else { /* spatial.py:1574-1577 */
+    float e[3];
+    for (int a = 0; a < 3; ++a) e[a] = p[a] + fdiv(d[a], G->spacing_out[a]);
+    for (int a = 0; a < 3; ++a) q[a] = affine_row(m + 4 * a, e[0], e[1], e[2]);
+  }
+  /* normalise (spatial.py:1646) then ATen un-normalise */
+  float u[3];
+  for (int a = 0; a < 3; ++a) {
+    float gn = fdiv(2.0f * q[a], G->nm1[a]) - 1.0f;
+    u[a] = ((gn + 1.0f) / 2.0f) * G->sm1[a];
+  }
+  /* trilinear corner weights (always needed for the mask) */
+  float fl0[3], lo[3], hi[3]; int64_t c0[3];
+  for (int a = 0; a < 3; ++a) {
+    fl0[a] = floorf(u[a]);
+    c0[a] = (int64_t)fl0[a];
+    lo[a] = (float)(c0[a] + 1) - u[a]; /* weight of corner c0 */
+    hi[a] = u[a] - (float)c0[a];       /* weight of corner c0+1 */
+  }
+  /* ATen order: x(=i) fastest, then y(=j), then z(=k); weight =
+   * (wx*wy)*wz; accumulate mul-then-add from 0 over in-bounds corners */
+  for (int t = 0; t < 8; ++t) {
+    int di = t & 1, dj = (t >> 1) & 1, dk = (t >> 2) & 1;
+    float wi = di ? hi[0] : lo[0], wj = dj ? hi[1] : lo[1], wk = dk ? hi[2] : lo[2];
+    v->w8[t] = (wi * wj) * wk;
+    int64_t ci = c0[0] + di, cj = c0[1] + dj, ck = c0[2] + dk;
+    v->inb[t] = ci >= 0 && ci < I && cj >= 0 && cj < J && ck >= 0 && ck < K;
+    v->off8[t] = (ci * J + cj) * K + ck;
+  }
+  v->use_fill = 0;
+  if (G->has_fill) {
+    float msum = 0.0f;
+    for (int t = 0; t < 8; ++t) if (v->inb[t]) msum = msum + 1.0f * v->w8[t];
+    v->use_fill = !(msum > 0.5f);
+  }
+  v->nn_off = -1;
+  if (G->mode == 0) { /* nearest: round-half-even */
+    int64_t r[3]; int ok_in = 1;
+    for (int a = 0; a < 3; ++a) {
+      r[a] = (int64_t)nearbyintf(u[a]);
+      if (r[a] < 0 || r[a] >= dims[a]) ok_in = 0;
+    }
+    if (ok_in) v->nn_off = (r[0] * J + r[1]) * K + r[2];
+  }
+}
+
 int orc_resample(const void* src, void* dst, int dtype,
                  int B, int C, int I, int J, int K,
                  int OI, int OJ, int OK,
@@ -132,12 +234,8 @@ int orc_resample(const void* src, void* dst, int dtype,
                  int affine_first, int mode, const float* fill) {
   const int64_t n_in = (int64_t)I * J * K, n_out = (int64_t)OI * OJ * OK;
   const size_t es = dtype_size(dtype);
-  /* max(size-1, 1) (spatial.py:1638-1640) */
-  const float nm1[3] = {(float)(I - 1 > 1 ? I - 1 : 1), (float)(J - 1 > 1 ? J - 1 : 1),
-                        (float)(K - 1 > 1 ? K - 1 : 1)};
-  /* ATen un-normalise multiplies by (size - 1) without the max() */
-  const float sm1[3] = {(float)(I - 1), (float)(J - 1), (float)(K - 1)};
-  const int dims[3] = {I, J, K};
+  const orc_geom G = geom_of(I, J, K, OI, OJ, OK, ni, nj, nk, spacing_in, spacing_out,
+                             affine_first, mode, fill != NULL);
   for (int b = 0; b < B; ++b) {
     const uint8_t fl = flags ? flags[b] : 0;
     if (fl & 1u) { /* pass-through row: exact copy (spatial.py:1101-1106) */
@@ -150,83 +248,90 @@ int orc_resample(const void* src, void* dst, int dtype,
     for (int oi = 0; oi < OI; ++oi)
       for (int oj = 0; oj < OJ; ++oj)
         for (int ok = 0; ok < OK; ++ok) {
-          float p[3] = {(float)oi, (float)oj, (float)ok};
-          float d[3] = {0.f, 0.f, 0.f};
-          if (g) { /* spatial.py:2171-2189 */
-            int i0, i1, j0, j1, k0, k1; float a0, a1, b0, b1, c0, c1;
-            lerp_setup(ni, OI, oi, &i0, &i1, &a0, &a1);
-            lerp_setup(nj, OJ, oj, &j0, &j1, &b0, &b1);
-            lerp_setup(nk, OK, ok, &k0, &k1, &c0, &c1);
-            for (int a = 0; a < 3; ++a)
-              d[a] = trilerp(g + a, nj, nk, 3, i0, i1, a0, a1, j0, j1, b0, b1,
-                             k0, k1, c0, c1);
-          }
-          float q[3];
-          if (!g) {
-            for (int a = 0; a < 3; ++a) q[a] = affine_row(m + 4 * a, p[0], p[1], p[2]);
-          } else if (affine_first) { /* spatial.py:1570-1573 */
-            for (int a = 0; a < 3; ++a)
-              q[a] = affine_row(m + 4 * a, p[0], p[1], p[2]) + fdiv(d[a], spacing_in[a]);
-          } else { /* spatial.py:1574-1577 */
-            float e[3];
-            for (int a = 0; a < 3; ++a) e[a] = p[a] + fdiv(d[a], spacing_out[a]);
-            for (int a = 0; a < 3; ++a) q[a] = affine_row(m + 4 * a, e[0], e[1], e[2]);
-          }
-          /* normalise (spatial.py:1646) then ATen un-normalise */
-          float u[3];
-          for (int a = 0; a < 3; ++a) {
-            float gn = fdiv(2.0f * q[a], nm1[a]) - 1.0f;
-            u[a] = ((gn + 1.0f) / 2.0f) * sm1[a];
-          }
-          /* trilinear corner weights (always needed for the mask) */
-          float fl0[3], lo[3], hi[3]; int64_t c0[3];
-          for (int a = 0; a < 3; ++a) {
-            fl0[a] = floorf(u[a]);
-            c0[a] = (int64_t)fl0[a];
-            lo[a] = (float)(c0[a] + 1) - u[a]; /* weight of corner c0 */
-            hi[a] = u[a] - (float)c0[a];       /* weight of corner c0+1 */
-          }
-          /* ATen order: x(=i) fastest, then y(=j), then z(=k); weight =
-           * (wx*wy)*wz; accumulate mul-then-add from 0 over in-bounds corners */
-          float w8[8]; int inb[8]; int64_t off8[8];
-          for (int t = 0; t < 8; ++t) {
-            int di = t & 1, dj = (t >> 1) & 1, dk = (t >> 2) & 1;
-            float wi = di ? hi[0] : lo[0], wj = dj ? hi[1] : lo[1], wk = dk ? hi[2] : lo[2];
-            w8[t] = (wi * wj) * wk;
-            int64_t ci = c0[0] + di, cj = c0[1] + dj, ck = c0[2] + dk;
-            inb[t] = ci >= 0 && ci < I && cj >= 0 && cj < J && ck >= 0 && ck < K;
-            off8[t] = (ci * J + cj) * K + ck;
-          }
-          int use_fill = 0;
-          if (fill) {
-            float msum = 0.0f;
-            for (int t = 0; t < 8; ++t) if (inb[t]) msum = msum + 1.0f * w8[t];
-            use_fill = !(msum > 0.5f);
-          }
-          int64_t nn_off = -1;
-          if (mode == 0) { /* nearest: round-half-even */
-            int64_t r[3]; int ok_in = 1;
-            for (int a = 0; a < 3; ++a) {
-              r[a] = (int64_t)nearbyintf(u[a]);
-              if (r[a] < 0 || r[a] >= dims[a]) ok_in = 0;
-            }
-            if (ok_in) nn_off = (r[0] * J + r[1]) * K + r[2];
-          }
+          orc_voxel vx;
+          resample_voxel(&G, m, g, oi, oj, ok, &vx);
           const int64_t o_off = ((int64_t)oi * OJ + oj) * OK + ok;
           for (int c = 0; c < C; ++c) {
             const int64_t ibase = ((int64_t)b * C + c) * n_in;
             const int64_t obase = ((int64_t)b * C + c) * n_out;
             float v;
-            if (use_fill) {
+            if (vx.use_fill) {
               v = fill[c];
             } else if (mode == 0) {
-              v = nn_off >= 0 ? load_as_f32(src, dtype, ibase + nn_off) : 0.0f;
+              v = vx.nn_off >= 0 ? load_as_f32(src, dtype, ibase + vx.nn_off) : 0.0f;
             } else {
               v = 0.0f;
               for (int t = 0; t < 8; ++t)
-                if (inb[t]) v = v + load_as_f32(src, dtype, ibase + off8[t]) * w8[t];
+                if (vx.inb[t]) v = v + load_as_f32(src, dtype, ibase + vx.off8[t]) * vx.w8[t];
             }
             store_from_f32(dst, dtype, obase + o_off, v);
+          }
+        }
+  }
+  return 0;
+}
+
+/* Adjoint of orc_resample with respect to its fp32 input, in float64: for every input voxel,
+ * grad64 = sum of g * w over the output voxels that read it (g of the fp32 grad_out, w the
+ * forward's fp32 weight; product and sum in double), abs64 = sum of |g * w|, and count = the
+ * number of terms.  The reference's backward (grid_sampler_3d_backward, then torch.where) adds
+ * the same terms in fp32:
+ *   - a voxel the forward fills sends nothing (torch.where routes no gradient to it);
+ *   - nearest sends g to its rounded voxel when that voxel is inside the volume;
+ *   - linear sends g * w to every in-bounds corner, zero weights included, so a NaN or Inf g
+ *     reaches them as NaN (NaN * 0 and Inf * 0 are NaN in double as in fp32);
+ *   - a pass-through element copies g (the shapes must then be equal).
+ * grad64 / abs64 are (B, C, I, J, K) double, count (B, C, I, J, K) int32. */
+int orc_resample_adjoint(const float* grad_out, double* grad64, double* abs64, int32_t* count,
+                         int B, int C, int I, int J, int K, int OI, int OJ, int OK,
+                         const float* mat, const float* cp, const uint8_t* flags,
+                         int ni, int nj, int nk,
+                         const float* spacing_in, const float* spacing_out,
+                         int affine_first, int mode, const float* fill) {
+  const int64_t n_in = (int64_t)I * J * K, n_out = (int64_t)OI * OJ * OK;
+  const orc_geom G = geom_of(I, J, K, OI, OJ, OK, ni, nj, nk, spacing_in, spacing_out,
+                             affine_first, mode, fill != NULL);
+  memset(grad64, 0, (size_t)B * C * n_in * sizeof(double));
+  memset(abs64, 0, (size_t)B * C * n_in * sizeof(double));
+  memset(count, 0, (size_t)B * C * n_in * sizeof(int32_t));
+  for (int b = 0; b < B; ++b) {
+    const uint8_t fl = flags ? flags[b] : 0;
+    if (fl & 1u) {
+      if (n_in != n_out) return 1;
+      for (int64_t t = 0; t < (int64_t)C * n_in; ++t) {
+        const int64_t o = (int64_t)b * C * n_in + t;
+        grad64[o] = (double)grad_out[o];
+        abs64[o] = fabs((double)grad_out[o]);
+        count[o] = 1;
+      }
+      continue;
+    }
+    const float* m = mat + (size_t)b * 12;
+    const float* g = (cp && (fl & 2u)) ? cp + (size_t)b * ni * nj * nk * 3 : NULL;
+    for (int oi = 0; oi < OI; ++oi)
+      for (int oj = 0; oj < OJ; ++oj)
+        for (int ok = 0; ok < OK; ++ok) {
+          orc_voxel vx;
+          resample_voxel(&G, m, g, oi, oj, ok, &vx);
+          if (vx.use_fill) continue;
+          const int64_t o_off = ((int64_t)oi * OJ + oj) * OK + ok;
+          for (int c = 0; c < C; ++c) {
+            const int64_t ibase = ((int64_t)b * C + c) * n_in;
+            const double go = (double)grad_out[((int64_t)b * C + c) * n_out + o_off];
+            if (mode == 0) {
+              if (vx.nn_off < 0) continue;
+              grad64[ibase + vx.nn_off] += go;
+              abs64[ibase + vx.nn_off] += fabs(go);
+              count[ibase + vx.nn_off] += 1;
+              continue;
+            }
+            for (int t = 0; t < 8; ++t) {
+              if (!vx.inb[t]) continue;
+              const double p = go * (double)vx.w8[t];
+              grad64[ibase + vx.off8[t]] += p;
+              abs64[ibase + vx.off8[t]] += fabs(p);
+              count[ibase + vx.off8[t]] += 1;
+            }
           }
         }
   }

@@ -144,6 +144,51 @@ def spatial(images, params):
         ]
 
 
+def _geometry_args(mat, cp, flags, spacing_in, spacing_out):
+    mat = _f32(mat).reshape(-1, 12).contiguous()
+    cp_t = None if cp is None else _f32(cp).contiguous()
+    flags_t = None if flags is None else torch.as_tensor(np.asarray(flags, dtype=np.uint8)).contiguous()
+    ni, nj, nk = (0, 0, 0) if cp is None else tuple(cp_t.shape[1:4])
+    return mat, cp_t, flags_t, (ni, nj, nk), _f32(spacing_in), _f32(spacing_out)
+
+
+def resample(src, out_shape, mat, cp, flags, spacing_in, spacing_out, *, affine_first, mode, fill):
+    """orc_resample of fp32 ``src`` (B, C, I, J, K) onto ``out_shape``, with the packed tables of
+    include/tio_b200.h as host arrays: mat (B, 12), cp (B, ni, nj, nk, 3) or None, flags (B,) or
+    None; mode 0 nearest, 1 linear; fill (C,) or None (no mask step)."""
+    src = src.float().contiguous()
+    b, c = src.shape[:2]
+    out = torch.empty((b, c, *out_shape), dtype=torch.float32)
+    mat, cp_t, flags_t, grid, sp_in, sp_out = _geometry_args(mat, cp, flags, spacing_in, spacing_out)
+    fill_t = None if fill is None else _f32(fill).reshape(-1).contiguous()
+    rc = lib().orc_resample(_p(src), _p(out), 0, b, c, *src.shape[2:], *out_shape, _p(mat), _p(cp_t),
+                            _p(flags_t), *grid, _p(sp_in), _p(sp_out), int(bool(affine_first)), int(mode),
+                            _p(fill_t))
+    assert rc == 0
+    return out
+
+
+def resample_adjoint(grad_out, in_shape, mat, cp, flags, spacing_in, spacing_out, *, affine_first, mode,
+                     fill):
+    """orc_resample_adjoint: (grad64, abs64, count), each (B, C, *in_shape), for the fp32
+    ``grad_out`` (B, C, OI, OJ, OK) of `resample` with the same geometry.  grad64 = sum of g * w
+    in float64 over the output voxels reading an input voxel, abs64 = sum of |g * w|, count =
+    the number of terms.  Only whether ``fill`` is None matters."""
+    grad_out = torch.as_tensor(grad_out).float().contiguous()
+    b, c = grad_out.shape[:2]
+    shape = (b, c, *(int(v) for v in in_shape))
+    grad64 = torch.empty(shape, dtype=torch.float64)
+    abs64 = torch.empty(shape, dtype=torch.float64)
+    count = torch.empty(shape, dtype=torch.int32)
+    mat, cp_t, flags_t, grid, sp_in, sp_out = _geometry_args(mat, cp, flags, spacing_in, spacing_out)
+    fill_t = None if fill is None else _f32(fill).reshape(-1).contiguous()
+    rc = lib().orc_resample_adjoint(_p(grad_out), _p(grad64), _p(abs64), _p(count), b, c, *shape[2:],
+                                    *grad_out.shape[2:], _p(mat), _p(cp_t), _p(flags_t), *grid, _p(sp_in),
+                                    _p(sp_out), int(bool(affine_first)), int(mode), _p(fill_t))
+    assert rc == 0, "orc_resample_adjoint: a pass-through element needs equal input and output shapes"
+    return grad64, abs64, count
+
+
 # ---- intensity ---------------------------------------------------------------
 
 
