@@ -159,10 +159,10 @@ typedef struct {
   int64_t nn_off;
 } orc_voxel;
 
-static void resample_voxel(const orc_geom* G, const float* m, const float* g, int oi, int oj,
-                           int ok, orc_voxel* v) {
-  const int I = G->I, J = G->J, K = G->K;
-  const int dims[3] = {I, J, K};
+/* Input-voxel coordinates q of output voxel (oi, oj, ok) (spatial.py:1504-1579), before the
+ * grid's normalisation: the sampling points of K1 and of the B-spline pull. */
+static void voxel_coords(const orc_geom* G, const float* m, const float* g, int oi, int oj, int ok,
+                         float q[3]) {
   float p[3] = {(float)oi, (float)oj, (float)ok};
   float d[3] = {0.f, 0.f, 0.f};
   if (g) { /* spatial.py:2171-2189 */
@@ -173,7 +173,6 @@ static void resample_voxel(const orc_geom* G, const float* m, const float* g, in
     for (int a = 0; a < 3; ++a)
       d[a] = trilerp(g + a, G->nj, G->nk, 3, i0, i1, a0, a1, j0, j1, b0, b1, k0, k1, c0, c1);
   }
-  float q[3];
   if (!g) {
     for (int a = 0; a < 3; ++a) q[a] = affine_row(m + 4 * a, p[0], p[1], p[2]);
   } else if (G->affine_first) { /* spatial.py:1570-1573 */
@@ -184,6 +183,14 @@ static void resample_voxel(const orc_geom* G, const float* m, const float* g, in
     for (int a = 0; a < 3; ++a) e[a] = p[a] + fdiv(d[a], G->spacing_out[a]);
     for (int a = 0; a < 3; ++a) q[a] = affine_row(m + 4 * a, e[0], e[1], e[2]);
   }
+}
+
+static void resample_voxel(const orc_geom* G, const float* m, const float* g, int oi, int oj,
+                           int ok, orc_voxel* v) {
+  const int I = G->I, J = G->J, K = G->K;
+  const int dims[3] = {I, J, K};
+  float q[3];
+  voxel_coords(G, m, g, oi, oj, ok, q);
   /* normalise (spatial.py:1646) then ATen un-normalise */
   float u[3];
   for (int a = 0; a < 3; ++a) {
@@ -265,6 +272,34 @@ int orc_resample(const void* src, void* dst, int dtype,
                 if (vx.inb[t]) v = v + load_as_f32(src, dtype, ibase + vx.off8[t]) * vx.w8[t];
             }
             store_from_f32(dst, dtype, obase + o_off, v);
+          }
+        }
+  }
+  return 0;
+}
+
+/* The fp32 coordinates q (B, OI, OJ, OK, 3) at which orc_resample samples each output voxel, in
+ * input voxels before the grid's normalisation; pass-through elements get their own voxel's
+ * indices (they are copied, not sampled). */
+int orc_sampling_coords(float* q, int B, int OI, int OJ, int OK,
+                        const float* mat, const float* cp, const uint8_t* flags,
+                        int ni, int nj, int nk,
+                        const float* spacing_in, const float* spacing_out, int affine_first) {
+  /* the coordinates do not depend on the input's shape */
+  const orc_geom G = geom_of(1, 1, 1, OI, OJ, OK, ni, nj, nk, spacing_in, spacing_out,
+                             affine_first, 1, 0);
+  for (int b = 0; b < B; ++b) {
+    const uint8_t fl = flags ? flags[b] : 0;
+    const float* m = mat + (size_t)b * 12;
+    const float* g = (cp && (fl & 2u)) ? cp + (size_t)b * ni * nj * nk * 3 : NULL;
+    for (int oi = 0; oi < OI; ++oi)
+      for (int oj = 0; oj < OJ; ++oj)
+        for (int ok = 0; ok < OK; ++ok) {
+          float* out = q + ((((int64_t)b * OI + oi) * OJ + oj) * OK + ok) * 3;
+          if (fl & 1u) {
+            out[0] = (float)oi; out[1] = (float)oj; out[2] = (float)ok;
+          } else {
+            voxel_coords(&G, m, g, oi, oj, ok, out);
           }
         }
   }

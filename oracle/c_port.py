@@ -66,15 +66,16 @@ def _f32(x):
 # ---- spatial ---------------------------------------------------------------
 
 
-def spatial_tables(params, batch, shape, affine0):
-    """(mat[B,12], cp[B,ni,nj,nk,3]|None, flags[B], (ni,nj,nk)) or None if no-op."""
+def spatial_tables(params, batch, shape, affine0, a_out=None):
+    """(mat[B,12], cp[B,ni,nj,nk,3]|None, flags[B], (ni,nj,nk)) or None if no-op.  ``a_out``: the
+    target space's affine (spatial.py:1582-1601); with one, every element is resampled."""
     per_instance = "affine_matrix" in (params.get("_batched_keys") or [])
     if per_instance:
         mats, cps = params["affine_matrix"], params["control_points"]
     else:
         mats = [params["affine_matrix"]] * batch
         cps = [params["control_points"]] * batch
-    if all(m is None for m in mats) and all(c is None for c in cps):
+    if a_out is None and all(m is None for m in mats) and all(c is None for c in cps):
         return None
     mat = torch.zeros(batch, 12)
     flags = torch.zeros(batch, dtype=torch.uint8)
@@ -86,12 +87,12 @@ def spatial_tables(params, batch, shape, affine0):
     if grid_shape is not None:
         cp = torch.zeros(batch, *grid_shape, 3)
     for b in range(batch):
-        m = tp.output_to_input_matrix(affine0, affine0, mats[b])
+        m = tp.output_to_input_matrix(affine0, affine0 if a_out is None else a_out, mats[b])
         mat[b] = m[:3].reshape(12)
         if cps[b] is not None:
             cp[b] = torch.as_tensor(cps[b], dtype=torch.float32)
             flags[b] |= 2
-        if per_instance and mats[b] is None and cps[b] is None:
+        if a_out is None and per_instance and mats[b] is None and cps[b] is None:
             flags[b] |= 1
     return mat, cp, flags, grid_shape or (0, 0, 0)
 
@@ -166,6 +167,19 @@ def resample(src, out_shape, mat, cp, flags, spacing_in, spacing_out, *, affine_
                             _p(fill_t))
     assert rc == 0
     return out
+
+
+def sampling_coords(out_shape, mat, cp, flags, spacing_in, spacing_out, *, affine_first):
+    """orc_sampling_coords: the fp32 input-voxel coordinates (B, OI, OJ, OK, 3) at which `resample`
+    (and the B-spline pull, through the same chain) samples every output voxel, with the geometry
+    arguments of `resample`.  Pass-through elements get their own voxel indices."""
+    mat, cp_t, flags_t, grid, sp_in, sp_out = _geometry_args(mat, cp, flags, spacing_in, spacing_out)
+    b = mat.shape[0]
+    q = torch.empty((b, *(int(v) for v in out_shape), 3), dtype=torch.float32)
+    rc = lib().orc_sampling_coords(_p(q), b, *q.shape[1:4], _p(mat), _p(cp_t), _p(flags_t), *grid, _p(sp_in),
+                                   _p(sp_out), int(bool(affine_first)))
+    assert rc == 0
+    return q
 
 
 def resample_adjoint(grad_out, in_shape, mat, cp, flags, spacing_in, spacing_out, *, affine_first, mode,

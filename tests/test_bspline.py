@@ -135,3 +135,132 @@ def test_entry_points_refuse_bad_arguments_without_touching_the_gpu():
         with pytest.raises(RuntimeError, match=message):
             _native.call(*args)
     assert lib.tio_launch_count() == before
+
+
+# ---- the float64 references and bounds the GPU tests use ------------------------------------------
+
+def _geometries():
+    """(name, out_shape, mat, cp, flags, spacing_in, spacing_out, affine_first, (a_in, a_out, worlds, cps))"""
+    from oracle import torch_port as tp
+
+    fx = bc.load_fixture("bspline_affine_o3")
+    (step,) = bc.params_of(fx)
+    worlds = step["params"]["affine_matrix"]
+    rng = np.random.default_rng(4)
+    cp = rng.uniform(-2, 2, (2, 5, 6, 4, 3)).astype(np.float32)
+    cp[:, :1] = cp[:, -1:] = 0
+    a_in = np.diag([1.2, 0.9, 1.0, 1.0])
+    a_out = np.diag([2.0, 1.5, 0.8, 1.0])
+    a_out[:3, 3] = (0.4, -0.3, 0.2)
+    tilt = np.eye(4)
+    tilt[:3, :3] = tp.output_to_input_matrix(np.eye(4), np.eye(4), None)[:3, :3].numpy()
+    tilt[0, 1] = 0.05
+    return [
+        ("golden_affine", bc.SHAPE, bc.SHAPE, np.eye(4), np.eye(4), worlds, [None] * len(worlds), True),
+        ("elastic_affine_first", (13, 11, 9), (13, 11, 9), a_in, a_in, [tilt, None], list(cp), True),
+        ("elastic_affine_last", (13, 11, 9), (13, 11, 9), a_in, a_in, [tilt, None], list(cp), False),
+        ("target_space", (13, 11, 9), (7, 8, 12), a_in, a_out, [tilt, None], [None, None], True),
+    ]
+
+
+@pytest.mark.parametrize("geometry", _geometries(), ids=lambda g: g[0])
+def test_sampling_coords_equal_torch_port(geometry):
+    """The C oracle's coordinate export is the reference's sampling grid, bit for bit."""
+    from oracle import c_port, torch_port as tp
+
+    _, in_shape, out_shape, a_in, a_out, worlds, cps, affine_first = geometry
+    mat = np.stack([tp.output_to_input_matrix(a_in, a_out, w)[:3].reshape(12).numpy() for w in worlds])
+    flags = np.array([2 if c is not None else 0 for c in cps], np.uint8)
+    cp = None if all(c is None for c in cps) else np.stack([np.zeros_like(cps[0]) if c is None else c for c in cps])
+    q = c_port.sampling_coords(out_shape, mat, cp, flags, tp.spacing_of(a_in), tp.spacing_of(a_out),
+                               affine_first=affine_first)
+    for b, (w, c) in enumerate(zip(worlds, cps)):
+        want = tp.sampling_grid(in_shape, a_in, out_shape, a_out, w, c, affine_first)
+        assert torch.equal(q[b].view(torch.int32), want.contiguous().view(torch.int32))
+
+
+@pytest.mark.parametrize("order", bc.ORDERS)
+def test_banded_solve_equals_dense_and_scipy(order):
+    rng = np.random.default_rng(order)
+    for n in range(1, 201):
+        x = rng.standard_normal((n, 2))
+        dense = np.linalg.solve(bc.collocation(n, order), x) if n > 1 else x
+        assert np.max(np.abs(bc.banded_coefficients(x, order) - dense)) <= 1e-12 * max(1.0, np.abs(dense).max())
+    if order <= 5:
+        x = rng.standard_normal(51199)
+        want = ndimage.spline_filter1d(x, order=order, mode="reflect")
+        assert np.max(np.abs(bc.banded_coefficients(x[:, None], order)[:, 0] - want)) <= 1e-10
+
+
+def _float64_slack(c, E):
+    """Float64's own rounding in prefilter64 (its fp32 bound E scaled by 2^-53 / 2^-24, doubled) and
+    in the dense solve (well below 2^-44 of the coefficients for these sizes): the truncation term is
+    attained on the alternating line, so the comparison needs them."""
+    return 2.0**-28 * E + 2.0**-44 * np.max(np.abs(c))
+
+
+@pytest.mark.parametrize("order", bc.ORDERS)
+def test_prefilter64_is_the_collocation_solve_within_its_algorithmic_bound(order):
+    """The documented algorithm with the kernel's fp32 poles, gain and horizons, in float64, against
+    the dense solve: every n from 2 to 64 (both initial sums for every pole), longer axes, and 3-D."""
+    rng = np.random.default_rng(10 + order)
+    zs, _ = bc.kernel_poles(order)
+    for z in zs:  # the host's logf may differ from the device's by an ulp: far from an integer either way
+        assert 1e-3 < float(bc.horizon_quotient(z)) % 1 < 1 - 1e-3
+    worst = 0.0
+    for n in [*range(2, 65), 100, 200]:
+        x = rng.standard_normal((n, 4))
+        x[:, 3] = (np.arange(n) % 2) * 2.0 - 1.0  # the alternating line: the largest coefficients
+        c, E, A = bc._pass(x, np.zeros_like(x), np.zeros_like(x), order)
+        err = np.abs(c - np.linalg.solve(bc.collocation(n, order), x))
+        bound = A + _float64_slack(c, E)
+        assert np.all(err <= bound), (n, float(np.max(err / bound)))
+        worst = max(worst, float(np.max(err / bound)))
+    x = rng.standard_normal((2, 9, 70, 13))
+    c, E, A = bc.prefilter64(x, order)
+    assert np.all(np.abs(c - bc.coefficients(x, order)) <= A + _float64_slack(c, E))
+    print(f"[prefilter64 o{order}] max |c64 - collocation| / A = {worst:.3f}")
+
+
+def _mutation_inputs():
+    from oracle import c_port
+
+    i, j, k = np.meshgrid(*(np.arange(n, dtype=np.float64) for n in bc.SHAPE), indexing="ij")
+    smooth = np.sin(i / 3) * np.cos(j / 4) + 0.5 * np.sin(k / 2)
+    noise = np.random.default_rng(5).standard_normal(bc.SHAPE)
+    rng = np.random.default_rng(6)
+    c = (np.asarray(bc.SHAPE) - 1) / 2
+    a = np.eye(3) + rng.uniform(-0.12, 0.12, (3, 3))
+    mat = np.concatenate([a, (c - a @ c + rng.uniform(-1, 1, 3))[:, None]], axis=1).astype(np.float32)
+    q = c_port.sampling_coords(bc.SHAPE, mat.reshape(1, 12), None, None, (1, 1, 1), (1, 1, 1),
+                               affine_first=True)[0].numpy().reshape(-1, 3)
+    return {"smooth": smooth, "noise": noise}, q
+
+
+@pytest.mark.parametrize("order", bc.ORDERS)
+def test_wrong_splines_leave_the_bound(order, monkeypatch):
+    """Three deliberately wrong float64 splines each leave the end-to-end bound somewhere, on smooth
+    and on noise input: the bounds are tight enough to see a subtly wrong kernel."""
+    inputs, q = _mutation_inputs()
+    for kind, x in inputs.items():
+        x32 = x.astype(np.float32).astype(np.float64)[None]
+        value, bound, inside = bc.end_to_end(x32, q, order)
+        c = bc.prefilter64(x32, order)[0]
+        shape = bc.SHAPE
+
+        def leaves(v):
+            return float(np.max(np.abs(v - value)[:, inside] / bound[:, inside]))
+
+        with monkeypatch.context() as m:  # the smallest Cox-de Boor weight dropped
+            cdb = bc.cox_de_boor
+            m.setattr(bc, "cox_de_boor", lambda g, o: cdb(g, o) * (np.arange(o + 1) != 0))
+            dropped = bc.tap_sums(q, order, shape, c)[0]
+        with monkeypatch.context() as m:  # the outermost tap folded as dct1 (-1 -> 1, n -> n - 2)
+            fold = bc.fold
+            m.setattr(bc, "fold", lambda t, n: np.where(t == -1, 1 % n, np.where(t == n, max(n - 2, 0),
+                                                                                  fold(t, n))))
+            dct1_tap = bc.tap_sums(q, order, shape, c)[0]
+        mirrored = bc.tap_sums(q, order, shape, bc.prefilter64(x32, order, mirror="dct1")[0])[0]
+        ratios = [leaves(dropped), leaves(dct1_tap), leaves(mirrored)]
+        print(f"[mutations o{order} {kind}] largest |wrong - right| / bound: " + ", ".join(f"{r:.3g}" for r in ratios))
+        assert min(ratios) > 1, ratios

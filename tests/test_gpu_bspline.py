@@ -1,6 +1,7 @@
-"""B-spline orders 2-7 on the GPU: the reference's fixtures, accuracy against the float64
-restatement, the exact cases (mask, passthrough, short axes, NaN), the public paths and the launch
-counts."""
+"""B-spline orders 2-7 on the GPU: the reference's fixtures within the per-voxel end-to-end bound of
+tests/bspline_cases.py (label mode by its float64 margins), the exact cases (mask, passthrough,
+NaN), the public paths and the launch counts.  Every kernel path against float64 is in
+tests/test_gpu_bspline_paths.py."""
 
 from __future__ import annotations
 
@@ -25,14 +26,6 @@ def _batch(data, seg=None):
     return tio.SubjectsBatch.from_subjects(subjects)
 
 
-def _tolerance(order) -> float:
-    """Share of the output's range: fp32 error of the prefilter grows with its gain (2, 3, 4.8, 7.5,
-    11.8, 18.5 per axis for orders 2-7); 64 roundings of 2^-24 amplified by the three axes' gains
-    bound the orders 6-7."""
-    gain = {2: 2.0, 3: 3.0, 4: 4.8, 5: 7.5, 6: 11.8, 7: 18.5}[order]
-    return 1e-4 if order <= 5 else 64 * 2.0**-24 * gain**3
-
-
 @pytest.mark.parametrize("name", list(bc.CASES))
 def test_fixture(name):
     case = bc.CASES[name]
@@ -52,8 +45,8 @@ def test_fixture(name):
         kwargs = case["kwargs"]
         order_name = kwargs.get("image_interpolation", "linear") if key == "t1" else kwargs["label_interpolation"]
         if order_name == "label":
-            if want.shape[1] == 1:  # argmax of fp32 channels: ties may break differently, rarely
-                assert np.mean(got != want) < 0.01
+            if want.shape[1] == 1:
+                _check_label_decisions(case, got, want)
             else:
                 np.testing.assert_allclose(got, want, atol=1e-4)
             continue
@@ -62,26 +55,75 @@ def test_fixture(name):
             assert np.max(np.abs(got.astype(np.float64) - want)) <= 1e-4 * span
             continue
         order = {**{v: k for k, v in bc.NAMES.items()}, **{o: o for o in bc.ORDERS}}[order_name]
-        if np.issubdtype(want.dtype, np.integer):
-            exact = bc.replay(case, exact=True)[key]["data"].numpy()
-            _assert_integer_exact(got, want, exact, order)
-        else:
-            span = max(float(np.ptp(want)), 1e-6)
-            assert np.max(np.abs(got.astype(np.float64) - want)) <= _tolerance(order) * span
+        data = t1 if key == "t1" else seg
+        if not bc.params_of(fx):  # every element gated out
+            assert np.array_equal(got, data.numpy())
+            continue
+        (step,) = bc.params_of(fx)
+        source, error = _antialiased(data, step["params"]) if kwargs.get("antialias") and key == "t1" else (None, None)
+        ratio = bc.check_end_to_end(data, torch.from_numpy(got), step["params"], order, source, error)
+        if got.dtype.kind == "f":
+            print(f"[fixture {name} {key}] max |gpu - ref| / bound = {ratio:.3f}")
+        else:  # most voxels must fall under the exact-equality rule, or it checks nothing
+            assert ratio < 0.5, ratio
+            print(f"[fixture {name} {key}] share within the bound of an integer = {ratio:.3f}")
 
 
-def _assert_integer_exact(got, want, exact, order):
-    """Integer outputs truncate the fp32 spline value: within 1 of the reference everywhere, and
-    equal wherever the float64 value is further from an integer than 1e-3 or the fp32 error bound
-    (8 roundings of 2^-24 of the largest value, amplified by the three axes' prefilter gains)."""
-    gain = {2: 2.0, 3: 3.0, 4: 4.8, 5: 7.5, 6: 11.8, 7: 18.5}[order]
-    thr = max(1e-3, 8 * 2.0**-24 * gain**3 * float(np.max(np.abs(exact))))
-    diff = got.astype(np.int64) - want.astype(np.int64)
-    assert np.max(np.abs(diff)) <= 1
-    away = np.abs(exact - np.round(exact)) > thr
-    assert away.mean() > 0.5, away.mean()
-    bad = away & (diff != 0)
-    assert not bad.any(), (int(bad.sum()), exact[bad][:5], got[bad][:5], want[bad][:5])
+def _antialiased(data, params):
+    """The anti-alias blur of the reference (torch_port) and a bound on how far the GPU's blur of the
+    same data may lie from it, gamma_m of the blur of |data|.  Per blurred axis of radius r, each side
+    rounds its 2r+1 weights (x / sigma, the square, exp counted as 2, the sum of 2r+1 weights and the
+    division: 2r + 5) and its sum of 2r+1 products (2r+1), all terms non-negative; m adds 4r + 6 per
+    axis for the host and again for the device.  The factor 1 + 2^-10 covers the fp32 rounding of
+    the blurred |data| itself."""
+    from oracle import torch_port as tp
+
+    a_out = np.asarray(params["target"]["affine"], dtype=np.float64)
+    sp_in = np.asarray(tp.spacing_of(np.eye(4)))
+    sigmas = tp.antialias_sigmas(np.asarray(tp.spacing_of(a_out)) / sp_in, sp_in)
+    radii = [max(int(np.ceil(3 * s)), 1) for s in sigmas if s > 0]
+    m = 2 * sum(4 * r + 6 for r in radii)
+    blurred = tp.antialias(data.float(), np.eye(4), a_out)
+    magnitude = tp.antialias(data.float().abs(), np.eye(4), a_out).double().numpy()
+    return blurred, bc.gamma(m) * magnitude * (1 + 2.0**-10)
+
+
+def _check_label_decisions(case, got, want):
+    """Label mode at C = 1 (argmax over one-hot splines, pad where their sum is not > 0.5): every
+    voxel whose |sum - 0.5| margin exceeds its bound, and, where the sum is above 0.5, whose top-two
+    margin exceeds its bound too, equals the float64 decision; the others are counted, and each holds
+    one of its near-tied labels."""
+    seg = bc.label_map(case)
+    (step,) = bc.params_of(bc.load_fixture(case["name"]))
+    params = step["params"]
+    order = {**{v: k for k, v in bc.NAMES.items()}}[params["one_hot_label_interpolation"]]
+    labels = torch.unique(seg)
+    onehot = (seg[:, 0][:, None] == labels.reshape(1, -1, 1, 1, 1)).float()
+    q, out_shape, flags = bc.step_coords(params, seg.shape[0], tuple(seg.shape[2:]))
+    pad = float(params["default_pad_label"])
+    undecided = 0
+    for e in range(seg.shape[0]):
+        value, bound, _ = bc.end_to_end(onehot[e].double().numpy(), q[e].reshape(-1, 3), order)
+        n = value.shape[0]
+        total = value.sum(axis=0)
+        total_bound = bound.sum(axis=0) + bc.gamma(n) * np.abs(value).sum(axis=0)
+        top = np.argsort(-value, axis=0, kind="stable")
+        v1 = np.take_along_axis(value, top[:1], 0)[0]
+        v2 = np.take_along_axis(value, top[1:2], 0)[0] if n > 1 else np.full_like(v1, -np.inf)
+        b1 = np.take_along_axis(bound, top[:1], 0)[0]
+        b2 = np.take_along_axis(bound, top[1:2], 0)[0] if n > 1 else np.zeros_like(v1)
+        # the argmax matters only where the sum says "inside"
+        decided = (np.abs(total - 0.5) > total_bound) & ((total < 0.5) | (v1 - v2 > b1 + b2))
+        decision = np.where(total > 0.5, labels.numpy()[top[0]], pad)
+        g = got[e, 0].reshape(-1).astype(np.float64)
+        assert np.array_equal(g[decided], decision[decided]), int((g[decided] != decision[decided]).sum())
+        near = value >= (v1 - b1)[None] - bound  # labels within the bounds of the top one
+        allowed = [set(labels.numpy()[near[:, p]].tolist()) | ({pad} if abs(total[p] - 0.5) <= total_bound[p] else set())
+                   for p in np.flatnonzero(~decided)]
+        for p, ok in zip(np.flatnonzero(~decided), allowed):
+            assert g[p] in ok, (p, g[p], ok)
+        undecided += int((~decided).sum())
+    print(f"[fixture {case['name']} label mode] {undecided} voxels within their bounds of a tie")
 
 
 def _affine_points(mat, shape):
@@ -117,37 +159,6 @@ def _pull(data, mats, order, flags=None, out_shape=None):
                                 order=order, out_shape=out_shape)
 
 
-@pytest.mark.parametrize("kind", ["noise", "smooth", "checkerboard"])
-@pytest.mark.parametrize("order", bc.ORDERS)
-def test_accuracy_against_float64(order, kind):
-    shape = (64, 64, 64)
-    g = torch.Generator().manual_seed(order)
-    if kind == "noise":
-        x = torch.randn(2, 1, *shape, generator=g, dtype=torch.float64)
-    elif kind == "smooth":
-        i, j, k = torch.meshgrid(*(torch.arange(n, dtype=torch.float64) for n in shape), indexing="ij")
-        x = (torch.sin(i / 5) * torch.cos(j / 7) + torch.sin(k / 3))[None, None].repeat(2, 1, 1, 1, 1)
-    else:
-        i, j, k = torch.meshgrid(*(torch.arange(n) for n in shape), indexing="ij")
-        x = ((i + j + k) % 2).double()[None, None].repeat(2, 1, 1, 1, 1)
-    x32 = x.float()
-    mats = _mats(2, shape, order)
-    got = _pull(x32.cuda(), mats, order).cpu().numpy().astype(np.float64)
-    hi = np.asarray(shape) - 1 + 0.05
-    for b in range(2):
-        pts = _affine_points(mats[b], shape)
-        want = bc.reference_pull(x32[b].double().numpy(), pts, order)
-        # the host restates the kernel's fp32 coordinate chain up to double rounding: leave the
-        # voxels within 1e-3 of the mask's edges to test_mask_bounds_are_strict
-        clear = np.all((np.abs(pts + 0.05) > 1e-3) & (np.abs(pts - hi) > 1e-3), axis=-1)
-        span = float(np.ptp(want))
-        err = np.abs(got[b] - want)[0][clear]
-        assert np.max(err) <= _tolerance(order) * span, (np.max(err), np.unravel_index(
-            np.argmax(np.abs(got[b] - want)[0] * clear), shape))
-        inside = np.all((pts > -0.05) & (pts < hi), axis=-1)
-        assert np.all(got[b][0][~inside & clear] == 0)
-
-
 def test_mask_bounds_are_strict():
     shape = (6, 6, 6)
     data = torch.ones(1, 1, *shape, device="cuda")
@@ -167,20 +178,11 @@ def test_u8_overshoot_truncates_like_the_reference():
     exact = bc.replay(case, exact=True)["t1"]["data"].numpy()
     assert (exact < -0.5).any() and (exact > 255.5).any()
     torch.manual_seed(bc.seed(case))
-    out = tio.Affine(**case["kwargs"])(_batch(bc.scalar_image(case).cuda())).images["t1"].data.cpu().numpy()
-    _assert_integer_exact(out, want, exact, 3)
-
-
-@pytest.mark.parametrize("shape", [(1, 5, 6), (2, 3, 7), (3, 1, 2), (2, 2, 1), (1, 1, 1), (1, 2, 2100)])
-@pytest.mark.parametrize("order", [3, 7])
-def test_short_axes(shape, order):
-    x = torch.randn(2, 2, *shape, generator=torch.Generator().manual_seed(3))
-    mats = np.stack([np.concatenate([np.eye(3), np.full((3, 1), 0.02)], axis=1)] * 2).astype(np.float32)
-    mats[1, :, 3] = -0.03
-    got = _pull(x.cuda(), mats, order).cpu().numpy()
-    for b in range(2):
-        want = bc.reference_pull(x[b].double().numpy(), _affine_points(mats[b], shape), order)
-        assert np.max(np.abs(got[b] - want)) <= _tolerance(order) * max(float(np.ptp(want)), 1.0)
+    out = tio.Affine(**case["kwargs"])(_batch(bc.scalar_image(case).cuda())).images["t1"].data.cpu()
+    assert np.max(np.abs(out.numpy().astype(np.int64) - want.astype(np.int64))) <= 1
+    (step,) = bc.params_of(bc.load_fixture("bspline_cubic_uint8"))
+    near = bc.check_end_to_end(bc.scalar_image(case), out, step["params"], 3)
+    assert near < 0.5, near  # most voxels fall under the exact-equality rule
 
 
 def test_passthrough_rows_are_bit_exact_and_skip_the_prefilter():
