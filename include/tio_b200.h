@@ -261,6 +261,7 @@ int tio_upload(const void* host_pinned, void* dst_device, size_t bytes, void* st
  * Per-channel minimum of batch element 0 -> fill[C] on the device, no host
  * sync.  Replaces _batch_fill_value("minimum") = tensor.min().item()
  * (spatial.py:2054-2060, 2094-2095).  `src` is (B, C, n) fp32, n = I*J*K.
+ * As torch.amin: NaN when the channel holds a NaN, otherwise its least value.
  */
 int tio_min_sample0(const float* src, int C, int64_t n, float* fill, void* stream);
 
@@ -312,8 +313,9 @@ int tio_randn_mt19937(uint64_t seed, uint64_t offset, uint64_t n, float* z,
  * Data-derived parameters of Standardize / Normalize, computed where the batch lives
  * (the reference reads batch element 0 on the host: standardize.py:52-79, normalize.py:121-139,
  * 332-366, _statistics.py:11-45).
- *   tio_moments    out3 (device doubles) = {sum, sum of squares, count} of the `n` values at `src`
- *                  for which mask[t] != 0 (mask NULL = all); fp64 accumulation, one pass
+ *   tio_moments    out3 (device doubles) = {sum, sum of (x - sum/count)^2, count} of the `n` values
+ *                  at `src` for which mask[t] != 0 (mask NULL = all); fp64 accumulation, two passes
+ *                  (the second reads the mean on the device), so a constant selection gives 0
  *   tio_quantiles  for each of the m <= 2 quantiles q (host doubles in [0,1]): index = q*(count-1),
  *                  lower = floor(index); values[2t], values[2t+1] = the order statistics of rank
  *                  lower and min(lower+1, count-1) (what torch.kthvalue(lower+1 / lower+2) returns),

@@ -81,10 +81,11 @@ def test_quantile_select_and_moments_match_torch_on_a_large_volume():
             want_hi = float(torch.kthvalue(values, min(lower + 2, values.numel())).values)
             assert vals[2 * t] == want_lo and vals[2 * t + 1] == want_hi
             assert weights[t] == pytest.approx(index - lower, abs=1e-9)
-        s, ss, n = ops.moments(x.cuda(), None if m is None else m.cuda())
+        s, dev, n = ops.moments(x.cuda(), None if m is None else m.cuda())
         assert n == values.numel()
         assert s / n == pytest.approx(float(values.double().mean()), rel=1e-12, abs=1e-12)
-        assert (ss - s * s / n) / (n - 1) == pytest.approx(float(values.double().var()), rel=1e-9)
+        # the second value is the sum of squared deviations from the mean, with no raw-moment cancellation
+        assert dev / (n - 1) == pytest.approx(float(values.double().var()), rel=1e-12)
     v, w, c = ops.quantile_neighbours(x.cuda(), [0.0, 1.0])
     assert v[0] == float(flat.min()) and v[2] == float(flat.max()) and w == [0.0, 0.0]
 

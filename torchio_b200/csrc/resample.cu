@@ -112,12 +112,22 @@ static int launch_typed(const ResampleArgs& a, int mode, cudaStream_t st) {
 
 // ---- min of sample 0 (fill value "minimum") --------------------------------
 
+// torch.amin's order: NaN wins, otherwise the least value (one instruction, as fminf)
+__device__ __forceinline__ float min_nan(float a, float b) {
+  float r;
+  asm("min.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+
+// valid for any mix of signs once *addr was initialised to +inf.  Dispatch on the sign bit: -0.0
+// takes the unsigned path, where it orders above +0.0 and below every negative.  A NaN is stored
+// as 0xffffffff, which wins both paths (the largest unsigned, a negative int) and reads as NaN.
 __device__ __forceinline__ void atomic_min_float(float* addr, float v) {
-  // valid for any mix of signs once *addr was initialised to +inf
-  if (v >= 0.0f)
-    atomicMin((int*)addr, __float_as_int(v));
+  const unsigned u = v != v ? 0xffffffffu : __float_as_uint(v);
+  if (u & 0x80000000u)
+    atomicMax((unsigned int*)addr, u);
   else
-    atomicMax((unsigned int*)addr, __float_as_uint(v));
+    atomicMin((int*)addr, (int)u);
 }
 
 __global__ void min_init_kernel(float* fill, int C) {
@@ -137,18 +147,18 @@ __global__ void __launch_bounds__(256) min_kernel(const float* __restrict__ src,
     const float4* p = (const float4*)base;
     for (int64_t t = t0; t < (n >> 2); t += stride) {
       float4 v = __ldg(p + t);
-      m = fminf(fminf(m, v.x), fminf(v.y, fminf(v.z, v.w)));
+      m = min_nan(min_nan(m, v.x), min_nan(min_nan(v.y, v.z), v.w));
     }
   } else {
-    for (int64_t t = t0; t < n; t += stride) m = fminf(m, __ldg(base + t));
+    for (int64_t t = t0; t < n; t += stride) m = min_nan(m, __ldg(base + t));
   }
 #pragma unroll
-  for (int s = 16; s > 0; s >>= 1) m = fminf(m, __shfl_xor_sync(0xffffffffu, m, s));
+  for (int s = 16; s > 0; s >>= 1) m = min_nan(m, __shfl_xor_sync(0xffffffffu, m, s));
   __shared__ float part[8];
   if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = m;
   __syncthreads();
   if (threadIdx.x == 0) {
-    for (int t = 1; t < 8; ++t) m = fminf(m, part[t]);
+    for (int t = 1; t < 8; ++t) m = min_nan(m, part[t]);
     atomic_min_float(fill + c, m);
   }
 }

@@ -8,7 +8,8 @@
 // and then applies `(x - mean) / std` or `(clamp(x) - in_min) / in_range * out_range + out_min`
 // as separate fp32 elementwise ops over the whole batch.
 //
-//   tio_moments    one pass: count, sum, sum of squares (fp64 accumulators) of the selected voxels
+//   tio_moments    two passes: count and sum, then the sum of squared deviations from their mean
+//                  (fp64 accumulators) of the selected voxels
 //   tio_quantiles_batched  exact order statistics of every batch element by a 3-level radix select
 //                  on the order-preserving integer image of fp32 (11 + 11 + 10 bits): three
 //                  streaming passes instead of a sort; returns the two neighbours of each quantile
@@ -24,8 +25,11 @@
 
 namespace tio {
 
+// ATen's radix key (TopKTypeConfig<float>): every NaN, whatever its sign, maps above +Inf, where
+// kthvalue puts it; key_value of that key is a NaN
 __device__ __forceinline__ uint32_t order_key(float x) {
   const uint32_t u = __float_as_uint(x);
+  if (x != x) return 0xffffffffu;
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 __device__ __forceinline__ float key_value(uint32_t k) {
@@ -33,9 +37,20 @@ __device__ __forceinline__ float key_value(uint32_t k) {
 }
 
 // ---- moments ---------------------------------------------------------------------------
+// Two passes, so that the variance does not come from raw moments: (ss - s*s/n) cancels when the
+// mean is large next to the spread and leaves rounding noise that depends on the order of the
+// atomics.  PASS 0 adds the sum and the count into out[0] and out[2]; PASS 1 reads the mean
+// out[0] / out[2] on the device and adds sum (x - mean)^2 into out[1].  A constant selection gives
+// exactly 0: its fp64 sum n*c is exact (c has 24 significant bits, n < 2^29), so mean == c.
+template <int PASS>
 __global__ void __launch_bounds__(256)
 moments_kernel(const float* __restrict__ src, const uint8_t* __restrict__ mask, int64_t n, double* out) {
-  double s = 0.0, ss = 0.0;
+  const double mean = PASS == 1 ? out[0] / out[2] : 0.0;
+  auto term = [&](float x) {
+    const double d = (double)x - mean;
+    return PASS == 0 ? d : d * d;
+  };
+  double s = 0.0;
   long long cnt = 0;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   const int64_t t0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -43,31 +58,32 @@ moments_kernel(const float* __restrict__ src, const uint8_t* __restrict__ mask, 
     const float4* p = reinterpret_cast<const float4*>(src);
     for (int64_t t = t0; t < (n >> 2); t += stride) {
       const float4 v = __ldg(p + t);
-      s += ((double)v.x + (double)v.y) + ((double)v.z + (double)v.w);
-      ss += ((double)v.x * v.x + (double)v.y * v.y) + ((double)v.z * v.z + (double)v.w * v.w);
+      s += (term(v.x) + term(v.y)) + (term(v.z) + term(v.w));
       cnt += 4;
     }
-    for (int64_t t = (n & ~(int64_t)3) + t0; t < n; t += stride) { const double v = src[t]; s += v; ss += v * v; ++cnt; }
+    for (int64_t t = (n & ~(int64_t)3) + t0; t < n; t += stride) { s += term(src[t]); ++cnt; }
   } else {
     for (int64_t t = t0; t < n; t += stride)
-      if (!mask || mask[t]) { const double v = src[t]; s += v; ss += v * v; ++cnt; }
+      if (!mask || mask[t]) { s += term(src[t]); ++cnt; }
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     s += __shfl_xor_sync(0xffffffffu, s, o);
-    ss += __shfl_xor_sync(0xffffffffu, ss, o);
-    cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+    if (PASS == 0) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
   }
-  __shared__ double ps[8], pss[8];
+  __shared__ double ps[8];
   __shared__ long long pc[8];
   const int w = threadIdx.x >> 5;
-  if ((threadIdx.x & 31) == 0) { ps[w] = s; pss[w] = ss; pc[w] = cnt; }
+  if ((threadIdx.x & 31) == 0) { ps[w] = s; pc[w] = cnt; }
   __syncthreads();
   if (threadIdx.x == 0) {
-    for (int t = 1; t < 8; ++t) { s += ps[t]; ss += pss[t]; cnt += pc[t]; }
-    atomicAdd(out + 0, s);
-    atomicAdd(out + 1, ss);
-    atomicAdd(out + 2, (double)cnt);
+    for (int t = 1; t < 8; ++t) { s += ps[t]; cnt += pc[t]; }
+    if (PASS == 0) {
+      atomicAdd(out + 0, s);
+      atomicAdd(out + 2, (double)cnt);
+    } else {
+      atomicAdd(out + 1, s);
+    }
   }
 }
 
@@ -423,7 +439,9 @@ extern "C" int tio_moments(const float* src, const uint8_t* mask, int64_t n, dou
   int blocks = (int)((n / 4 + 255) / 256);
   if (blocks > num_sms() * 8) blocks = num_sms() * 8;
   if (blocks < 1) blocks = 1;
-  moments_kernel<<<blocks, 256, 0, st>>>(src, mask, n, out3);
+  moments_kernel<0><<<blocks, 256, 0, st>>>(src, mask, n, out3);
+  launched();
+  moments_kernel<1><<<blocks, 256, 0, st>>>(src, mask, n, out3);
   launched();
   TIO_CHECK_LAUNCH();
   return 0;

@@ -468,7 +468,8 @@ def remap(src: Tensor, out_shape, offsets, *, mode: str = "constant", fill=0, fl
         if (tuple(dst.shape) != (b, c, oi, oj, ok) or dst.dtype != src.dtype or dst.device != src.device
                 or not dst.is_contiguous()):
             raise ValueError("remap: `out` must be a contiguous (B, C, *out_shape) block of the source's dtype/device")
-    fill_host = torch.tensor([fill]).to(src.dtype)  # F.pad casts the value to the tensor's dtype
+    # F.pad casts the value (a double) to the tensor's dtype: an fp64 tensor keeps all of it
+    fill_host = torch.tensor([fill], dtype=torch.float64 if isinstance(fill, float) else None).to(src.dtype)
     _launch("tio_remap", src.device, _ptr(src), _ptr(dst), src.element_size(), b, c, i, j, k, oi, oj, ok,
             int(offsets[0]), int(offsets[1]), int(offsets[2]), PAD_MODES[mode], fill_host.data_ptr(), _ptr(flip))
     return dst
@@ -516,9 +517,9 @@ WIDE_R = 16
 
 
 def moments(values: Tensor, mask: Tensor | None = None) -> tuple[float, float, float]:
-    """(sum, sum of squares, count) of the selected values of a contiguous fp32 CUDA tensor, fp64
-    accumulation on the device, one small D2H read (the reference calls ``.item()`` here too:
-    standardize.py:76-77)."""
+    """(sum, sum of squared deviations from the mean, count) of the selected values of a contiguous
+    fp32 CUDA tensor, fp64 accumulation on the device, one small D2H read (the reference calls
+    ``.item()`` here too: standardize.py:76-77)."""
     values = _batch(values, "moments", ndim=None)
     m8 = None if mask is None else mask.expand_as(values).contiguous().to(torch.uint8)
     out = torch.empty(3, dtype=torch.float64, device=values.device)

@@ -533,10 +533,10 @@ class Standardize(IntensityTransform):
             mask = _resolve_mask(self.masking_method, img_batch, batch)
             with _Staged(img_batch) as staged:
                 tensor, mask = _sample0(staged, mask, f'Mask is empty for "{name}". Using all voxels.')
-                s, ss, n = ops.moments(tensor, mask)
+                s, dev, n = ops.moments(tensor, mask)
             mean = s / n
-            var = (ss - s * s / n) / (n - 1) if n > 1 else float("nan")  # torch.std: Bessel's correction
-            stats[name] = (float(np.float32(mean)), float(np.float32(np.sqrt(max(var, 0.0)))))
+            var = dev / (n - 1) if n > 1 else float("nan")  # torch.std: Bessel's correction
+            stats[name] = (float(np.float32(mean)), float(np.float32(np.sqrt(var))))
         return {"stats": stats}
 
     def apply_transform(self, batch: SubjectsBatch, params: dict[str, Any]) -> SubjectsBatch:

@@ -11,6 +11,7 @@ origin, flip leaves the affine untouched).
 
 from __future__ import annotations
 
+import math
 import warnings
 from collections.abc import Sequence
 from typing import Any
@@ -202,7 +203,8 @@ def _padding_statistics(data, mode: str) -> list:
     """One whole-volume statistic per batch element (`_compute_padding_statistic`,
     _padding.py:41-68), computed where the batch lives: minimum = `tio_min_sample0` over the
     element, mean = `tio_moments` (fp64 sums; the reference's fp32 `mean()` agrees to rounding),
-    median = the exact radix select behind `compute_quantile(values, 0.5)`."""
+    median = the exact radix select behind `compute_quantile(values, 0.5)`.  fp64 data keeps its
+    mean and median in fp64 as the reference does, through torch's own ops (kthvalue + lerp)."""
     from .intensity import _lerp_f32
 
     b = data.shape[0]
@@ -211,6 +213,19 @@ def _padding_statistics(data, mode: str) -> list:
             mins = [ops.min_sample0(data[i:i + 1].reshape(1, 1, -1, 1, 1)) for i in range(b)]
             return torch.cat(mins).tolist()
         return data.flatten(start_dim=1).amin(dim=1).tolist()
+    if data.dtype == torch.float64:
+        flat = data.flatten(start_dim=1)
+        if mode == "mean":
+            return flat.mean(dim=1).tolist()
+        index = 0.5 * (flat.shape[1] - 1)
+        lower = math.floor(index)
+        values = []
+        for row in flat:
+            median = row.kthvalue(lower + 1).values
+            if index != lower:
+                median = median.lerp(row.kthvalue(lower + 2).values, index - lower)
+            values.append(float(median))
+        return values
     if not torch.is_floating_point(data):
         warnings.warn(
             f'The constant value computed for padding mode "{mode}"'
