@@ -292,13 +292,19 @@ int tio_blur(const float* src, float* dst, float* scratch,
  * K4a — exact replay of torch's CPU `randn` stream on the device:
  * mt19937(seed) -> 24-bit uniforms -> 16-wide Box-Muller blocks (ATen normal_fill;
  * the stream the reference depends on through torch.randn(generator=CPU),
- * noise.py:166-178).  Writes stream elements [offset, offset+n) to z[0..n).
- * Requires offset % 16 == 0, n % 16 == 0, n >= 16 (ragged tails and tiny draws
- * stay on the host), and offset + n <= 2^31 words.
+ * noise.py:166-178).
+ * tio_randn_mt19937_window: outputs [lo, hi) of torch.randn(n) drawn at stream word
+ * `offset` (after `offset` words of the generator were used), output i to z[i - lo].
+ * Any offset, any n >= 16, lo < hi <= n.  The draw takes words [offset, offset+n)
+ * in 16-groups relative to offset (u[j] pairs with u[j+8]); when n % 16 != 0 it then
+ * takes 16 more words, which give outputs [n-16, n) anew, so it ends at word
+ * offset + n + 16 (offset + n otherwise), at most 2^31.
+ * tio_randn_mt19937: the [0, n) window, for offset % 16 == 0, n % 16 == 0, n >= 16.
  *   table      device copy of the jump-ahead table built once by
  *              tio_mt19937_build_table (host, ~2 s; depends only on MT19937, so
  *              callers cache it; tio_mt19937_table_bytes() gives its size)
- *   workspace  device scratch of tio_randn_mt19937_workspace_bytes(offset, n)
+ *   workspace  device scratch of tio_randn_mt19937_workspace_bytes(offset, n), or of
+ *              tio_randn_mt19937_window_workspace_bytes(offset, n) for the window
  * The uniforms are bit-identical to torch.s; normals agree to <= 4e-6 absolute
  * (CUDA libm vs the host.s log/sin/cos).
  */
@@ -308,6 +314,10 @@ size_t tio_randn_mt19937_workspace_bytes(uint64_t offset, uint64_t n);
 int tio_randn_mt19937(uint64_t seed, uint64_t offset, uint64_t n, float* z,
                       const void* table, void* workspace, size_t workspace_bytes,
                       void* stream);
+size_t tio_randn_mt19937_window_workspace_bytes(uint64_t offset, uint64_t n);
+int tio_randn_mt19937_window(uint64_t seed, uint64_t offset, uint64_t n, uint64_t lo, uint64_t hi,
+                             float* z, const void* table, void* workspace, size_t workspace_bytes,
+                             void* stream);
 
 /*
  * Data-derived parameters of Standardize / Normalize, computed where the batch lives

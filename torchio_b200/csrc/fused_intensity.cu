@@ -934,17 +934,18 @@ march6_kernel(const float* __restrict__ src, float* __restrict__ dst, int B, int
 //                   tiles (k-block, j-block, b*c) of that kernel's grid, x fastest, handed out by
 //                   a global counter;
 //   warpgroups 2-6  lowered to 40 registers: the first MT_THREADS threads run segment after
-//                   segment of the normal stage (q = q_lo + blockIdx.x, + gridDim.x, ...), the
-//                   other 64 leave;
+//                   segment of the normal stage compiled for aligned [0, n) draws
+//                   (q = q_lo + blockIdx.x, + gridDim.x, ...), the other 64 leave;
 // 256 x 152 + 640 x 40 = 64 512 registers after the exchange.  Both bodies are the device
-// functions the stand-alone kernels run, so the outputs are theirs bit for bit.  Named barriers:
+// functions the stand-alone kernels run (the normal stage with the same Box-Muller arithmetic),
+// so the outputs are theirs bit for bit.  Named barriers:
 // 1..5 inside the normal stage, P1N_BAR_SEGMENT between its segments, P1N_BAR_MARCH for pass 1;
 // barrier 0 is never used after the roles part.
 // -------------------------------------------------------------------------
 constexpr int P1N_MARCH_THREADS = 256;
 constexpr int P1N_THREADS = P1N_MARCH_THREADS + 5 * 128;  // 896
 constexpr int P1N_BAR_SEGMENT = 6, P1N_BAR_MARCH = 7;
-constexpr int P1N_RING_FLOATS = MT_RING * MT_N + 4;  // the normal stage's ring, then the tile slot
+constexpr int P1N_RING_FLOATS = MT_RING_WORDS + 4;  // the normal stage's ring, then the tile slot
 
 template <bool HAS_BIAS>
 __global__ void __launch_bounds__(P1N_THREADS, 1)
@@ -956,7 +957,7 @@ pass1_normals_kernel(const float* __restrict__ src, float* __restrict__ dst, int
   if (threadIdx.x < P1N_MARCH_THREADS) {
     asm volatile("setmaxnreg.inc.sync.aligned.u32 152;");
     const int tid = threadIdx.x;
-    volatile int* next_tile = reinterpret_cast<int*>(smem + MT_RING * MT_N);
+    volatile int* next_tile = reinterpret_cast<int*>(smem + MT_RING_WORDS);
     const int kb_n = (K + 255) / 256, jb_n = (J + 3) / 4;
     const int tiles = kb_n * jb_n * B * C;
     for (;;) {
@@ -975,7 +976,7 @@ pass1_normals_kernel(const float* __restrict__ src, float* __restrict__ dst, int
     const int tid = threadIdx.x - P1N_MARCH_THREADS;
     if (tid >= MT_THREADS) return;
     for (int q = q_lo + blockIdx.x; q < q_hi; q += gridDim.x) {
-      mt_normal_segment(reinterpret_cast<uint32_t*>(smem), tid, states, q, L, offset, n, z);
+      mt_normal_segment<false>(reinterpret_cast<uint32_t*>(smem), tid, states, q, L, offset, n, 0, n, z);
       // the last consumers have left the ring before the next segment's start state enters it
       mt_bar_sync<P1N_BAR_SEGMENT, MT_THREADS>();
     }
@@ -1302,12 +1303,15 @@ extern "C" int tio_intensity_pass1_with_normals(const float* src, float* dst, in
                   "%s: coarse bias grid empty or too large", who);
   }
   BlurArgs bl{need_i ? taps : nullptr, radius, R};
+  TIO_CHECK_ARG(n >= 16 && (n % 16) == 0 && (offset % 16) == 0, "%s: n and offset must be multiples of 16 (n >= 16)",
+                who);
   TIO_CHECK_ARG(workspace_bytes >= tio_intensity_pass1_with_normals_workspace_bytes(offset, n),
                 "%s: workspace too small", who);
   cudaStream_t st = (cudaStream_t)stream;
   int q_lo, q_hi;
   const size_t states_bytes = tio_randn_mt19937_workspace_bytes(offset, n);
-  if (int rc = mt_start_states(seed, offset, n, table, workspace, states_bytes, st, who, &q_lo, &q_hi)) return rc;
+  if (int rc = mt_start_states(seed, offset, offset + n - 16, table, workspace, states_bytes, st, who, &q_lo, &q_hi))
+    return rc;
   unsigned int* tile_counter = reinterpret_cast<unsigned int*>((char*)workspace + states_bytes);
   cudaMemsetAsync(tile_counter, 0, sizeof(unsigned int), st);
   const int ns = coarse ? si * sj * sk : 0;

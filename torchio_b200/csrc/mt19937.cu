@@ -2,14 +2,18 @@
 //
 // torch.randn(shape, generator=CPU mt19937(seed)) (the reference's noise source,
 // transforms/intensity/noise.py:166-178) for n >= 16 is ATen's normal_fill:
-//   u[t]  = (mt19937_word[t] & 0xFFFFFF) * 2^-24                t = 0..n-1
+//   u[t]  = (mt19937_word[s + t] & 0xFFFFFF) * 2^-24            t = 0..n-1
 //   per 16-block, j = 0..7:  r = sqrt(-2 log(1 - u[j])),  th = 2*pi*u[j+8]
 //                            z[j] = r cos th,  z[j+8] = r sin th
-// one sequential stream per call.  Here the stream is cut into segments of
+//   n % 16 != 0: 16 more words u[n..n+16) as one more block, written to z[n-16..n)
+// where s is the number of words the generator used before; the calls of one generator
+// continue one sequential stream.  A draw may start at any word and only a window of its
+// outputs may be wanted (tio_randn_mt19937_window).  Here the stream is cut into segments of
 // L = 2^21 words (mt19937_layout.h); segment start states come from jump-ahead
 // polynomials (mt19937_jump.cpp): seed -> W_0, coarse jumps W_0 -> W_{m*S2*L}, fine
 // jumps -> W_{(S2*m+r)L}; then one CTA per segment regenerates its 624-word blocks
-// (three dependency waves of <= 227 words) and emits normals.
+// (three dependency waves of <= 227 words) and emits the normals of the 16-blocks whose
+// first word lies in the segment.
 //
 // Window W_t = (x[t], ..., x[t+623]) of the word recurrence
 //   x[k+624] = x[k+397] ^ twist(x[k], x[k+1]);  stream word t = temper(x[624+t]).
@@ -106,23 +110,23 @@ mt_jump_kernel(uint32_t* __restrict__ states, const uint16_t* __restrict__ polys
 
 // One CTA per segment q (the stage itself: mt19937_normal.cuh)
 __global__ void __launch_bounds__(MT_THREADS, 2)
-mt_normal_kernel(const uint32_t* __restrict__ states, int q_first, unsigned long long L,
-                 unsigned long long offset, unsigned long long n, float* __restrict__ z) {
-  __shared__ __align__(16) uint32_t ring[MT_RING * MT_N];
-  mt_normal_segment(ring, (int)threadIdx.x, states, q_first + (int)blockIdx.x, L, offset, n, z);
+mt_normal_kernel(const uint32_t* __restrict__ states, int q_first, unsigned long long L, unsigned long long s,
+                 unsigned long long n, unsigned long long lo, unsigned long long hi, float* __restrict__ z) {
+  __shared__ __align__(16) uint32_t ring[MT_RING_WORDS];
+  mt_normal_segment<true>(ring, (int)threadIdx.x, states, q_first + (int)blockIdx.x, L, s, n, lo, hi, z);
 }
 
 constexpr uint64_t MT_L = 1ull << tio_mt::kLog2L;
+constexpr uint64_t MT_MAX_WORDS = (uint64_t)tio_mt::kS1 * tio_mt::kS2 * MT_L;  // the table's reach
 
-int mt_start_states(uint64_t seed, uint64_t offset, uint64_t n, const void* table, void* workspace,
-                    size_t workspace_bytes, cudaStream_t st, const char* who, int* q_lo_out, int* q_hi_out) {
+int mt_start_states(uint64_t seed, uint64_t first_word, uint64_t last_word, const void* table,
+                    void* workspace, size_t workspace_bytes, cudaStream_t st, const char* who, int* q_lo_out,
+                    int* q_hi_out) {
   TIO_CHECK_ARG(table && workspace, "%s: null table or workspace", who);
-  TIO_CHECK_ARG(n >= 16 && (n % 16) == 0 && (offset % 16) == 0,
-                "%s: n and offset must be multiples of 16 (n >= 16)", who);
   const int S2 = tio_mt::kS2, S1 = tio_mt::kS1, stride = tio_mt::kStride;
-  const uint64_t q_lo = offset / MT_L, q_hi = (offset + n + MT_L - 1) / MT_L;  // segments [q_lo, q_hi)
+  const uint64_t q_lo = first_word / MT_L, q_hi = last_word / MT_L + 1;  // segments [q_lo, q_hi)
   TIO_CHECK_ARG(q_hi <= (uint64_t)S1 * S2, "%s: stream position beyond %d segments", who, S1 * S2);
-  TIO_CHECK_ARG(workspace_bytes >= tio_randn_mt19937_workspace_bytes(offset, n), "%s: workspace too small", who);
+  TIO_CHECK_ARG(workspace_bytes >= (size_t)(q_hi + S1) * MT_N * 4, "%s: workspace too small", who);
   uint32_t* states = (uint32_t*)workspace;
   const uint16_t* polys = (const uint16_t*)((const char*)table + tio_mt::kHeaderBytes);
   mt_seed_kernel<<<1, 32, 0, st>>>((uint32_t)seed, states);
@@ -157,18 +161,41 @@ extern "C" size_t tio_randn_mt19937_workspace_bytes(uint64_t offset, uint64_t n)
   return (size_t)(q_hi + tio_mt::kS1) * MT_N * 4;
 }
 
-extern "C" int tio_randn_mt19937(uint64_t seed, uint64_t offset, uint64_t n, float* z,
-                                 const void* table, void* workspace, size_t workspace_bytes,
-                                 void* stream) {
-  TIO_CHECK_ARG(z, "tio_randn_mt19937: null pointer");
+// q_hi = the segment of the last group's first word, + 1: the tail's s + n, or s + n - 16
+extern "C" size_t tio_randn_mt19937_window_workspace_bytes(uint64_t offset, uint64_t n) {
+  const uint64_t last = offset + ((n % 16) ? n : n - 16);
+  return (size_t)(last / MT_L + 1 + tio_mt::kS1) * MT_N * 4;
+}
+
+extern "C" int tio_randn_mt19937_window(uint64_t seed, uint64_t offset, uint64_t n, uint64_t lo, uint64_t hi,
+                                        float* z, const void* table, void* workspace, size_t workspace_bytes,
+                                        void* stream) {
+  const char* who = "tio_randn_mt19937_window";
+  TIO_CHECK_ARG(z, "%s: null pointer", who);
+  TIO_CHECK_ARG(n >= 16 && lo < hi && hi <= n, "%s: needs n >= 16 and lo < hi <= n", who);
+  const uint64_t words = n + ((n % 16) ? 16 : 0);  // the tail group takes 16 more words
+  TIO_CHECK_ARG(offset < MT_MAX_WORDS && words <= MT_MAX_WORDS - offset,
+                "%s: the draw ends beyond stream word 2^31", who);
+  // first words of the first and last groups with outputs in [lo, hi)
+  const uint64_t kept = (n % 16) ? n - 16 : n;  // outputs of the 16-groups the tail leaves
+  const uint64_t first = lo < kept ? offset + lo / 16 * 16 : offset + n;
+  const uint64_t last = hi > kept ? offset + n : offset + (hi - 1) / 16 * 16;
   cudaStream_t st = (cudaStream_t)stream;
   int q_lo, q_hi;
-  if (int rc = mt_start_states(seed, offset, n, table, workspace, workspace_bytes, st, "tio_randn_mt19937",
-                               &q_lo, &q_hi))
+  if (int rc = mt_start_states(seed, first, last, table, workspace, workspace_bytes, st, who, &q_lo, &q_hi))
     return rc;
   mt_normal_kernel<<<(unsigned)(q_hi - q_lo), MT_THREADS, 0, st>>>((const uint32_t*)workspace, q_lo, MT_L, offset,
-                                                                   n, z);
+                                                                   n, lo, hi, z);
   launched();
   TIO_CHECK_LAUNCH();
   return 0;
+}
+
+// the [0, n) window of an aligned draw
+extern "C" int tio_randn_mt19937(uint64_t seed, uint64_t offset, uint64_t n, float* z,
+                                 const void* table, void* workspace, size_t workspace_bytes,
+                                 void* stream) {
+  TIO_CHECK_ARG(n >= 16 && (n % 16) == 0 && (offset % 16) == 0,
+                "tio_randn_mt19937: n and offset must be multiples of 16 (n >= 16)");
+  return tio_randn_mt19937_window(seed, offset, n, 0, n, z, table, workspace, workspace_bytes, stream);
 }

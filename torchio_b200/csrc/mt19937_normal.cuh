@@ -73,46 +73,83 @@ __device__ __forceinline__ void mt_bar_arrive() {
   asm volatile("bar.arrive %0, %1;" ::"n"(ID), "n"(COUNT) : "memory");
 }
 
-// Normal stage layout.  MT_THREADS threads emit stream words [q*L, (q+1)*L) of segment q
-// intersected with [offset, offset+n) as z[word - offset].  Warp-specialised:
+// Normal stage layout.  MT_THREADS threads emit the 16-groups of a draw whose first word lies in
+// segment q (stream words [q*L, (q+1)*L)).  A draw of n normals at stream word s is torch's
+// normal_fill: groups of 16 words [s + 16g, s + 16g + 16) give outputs [16g, 16g + 16) (u[j] and
+// u[j+8] pair up); when n % 16 != 0 a tail group of the 16 words [s + n, s + n + 16) then gives
+// outputs [n - 16, n), overwriting what the last groups wrote there.  Only outputs [lo, hi) of
+// the draw are written, output i to z[i - lo].  A group belongs to the segment holding its first
+// word, so the last groups of a segment may read up to 15 words of the next one.
+// Warp-specialised:
 //   producers (8 warps) regenerate the segment's 624-word blocks in the recurrence's three
 //     dependency waves (227, 227, 170 words), synchronised among themselves only;
 //   consumers (10 warps) temper and transform them.  A consumer thread owns one "item" per
 //     round: half of a 16-group (pairs j0..j0+3, j0 = 0 or 4), i.e. four independent
-//     Box-Muller chains, read with two LDS.128 and written with two 16-byte stores.
+//     Box-Muller chains, read with two LDS.128 and written with two 16-byte stores where the
+//     draw's alignment allows (scalar accesses otherwise).  Each block holds the first words of
+//     39 groups; two of the otherwise idle consumers take the tail group.
 // Blocks pass in rounds of MT_ROUND blocks (= 312 items, one per consumer thread) through a
-// ring of two rounds: producers fill one round while consumers drain the other.  Named
-// barriers: MT_BAR_PROD among producers, MT_BAR_FULL + r and MT_BAR_EMPTY + r (round buffer
-// r) between the two roles.  Producers wait for consumers only when both buffers are full.
+// ring of two rounds: producers fill one round while consumers drain the other.  A round's
+// blocks are contiguous and followed by the first 16 words of the next block, so a group that
+// straddles two blocks, or two rounds, reads consecutive words.  Named barriers: MT_BAR_PROD
+// among producers, MT_BAR_FULL + r and MT_BAR_EMPTY + r (round buffer r) between the two roles.
+// Producers wait for consumers only when both buffers are full.
 constexpr int MT_ROUND = 4;                          // blocks per round
-constexpr int MT_RING = 2 * MT_ROUND;                // blocks in shared memory (19.5 KB)
+constexpr int MT_RING = 2 * MT_ROUND;                // blocks in the ring
+constexpr int MT_ROUND_WORDS = MT_ROUND * MT_N + 16;  // a round's blocks, then the next block's first 16 words
+constexpr int MT_RING_WORDS = 2 * MT_ROUND_WORDS;    // 5024 words (19.6 KB)
 constexpr int MT_ITEMS = MT_ROUND * MT_N / 8;        // 312 items per round
 constexpr int MT_PRODUCERS = 256;                    // >= 227 (one wave's width), whole warps
 constexpr int MT_CONSUMERS = (MT_ITEMS + 31) / 32 * 32;  // 320
 constexpr int MT_THREADS = MT_PRODUCERS + MT_CONSUMERS;  // 576
 constexpr int MT_BAR_PROD = 1, MT_BAR_FULL = 2, MT_BAR_EMPTY = 4;  // ids 1..5; none uses barrier 0
+static_assert(MT_CONSUMERS >= MT_ITEMS + 2, "the tail group needs two spare consumers");
 
-// `ring`: MT_RING * MT_N words of shared memory, 16-byte aligned (block b in slot b % MT_RING);
-// `tid` in [0, MT_THREADS).  Every barrier is balanced within the call, but the last consumers
-// may still read the ring when the producers return: a caller that runs a second segment puts a
-// barrier over the MT_THREADS threads between the two.
+// block b >= -1 of the segment (block -1: the start window) in the ring
+__device__ __forceinline__ uint32_t* mt_block(uint32_t* ring, int b) {
+  const int slot = (b + MT_RING) % MT_RING;
+  return ring + (slot / MT_ROUND) * MT_ROUND_WORDS + (slot % MT_ROUND) * MT_N;
+}
+
+// segment-relative positions, clamped to a range that keeps every comparison below exact
+__device__ __forceinline__ int mt_rel(long long v, unsigned long long L) {
+  return (int)min(max(v, -32ll), (long long)L + 32);
+}
+
+// `ring`: MT_RING_WORDS words of shared memory, 16-byte aligned; `tid` in [0, MT_THREADS).
+// The draw: n >= 16 normals at stream word s, outputs [lo, hi) with lo < hi <= n.
+// WINDOW = false compiles the stage for the [0, n) window of an aligned draw only (s and n
+// multiples of 16, lo = 0, hi = n, z 16-byte aligned): no group straddles a block, there is no
+// tail, and every item takes the 16-byte path, so the consumer loop carries none of the window's
+// bounds (pass1_normals_kernel, where this stage is the longer of the two roles).  Every
+// barrier is balanced within the call, but the last consumers may still read the ring when the
+// producers return: a caller that runs a second segment puts a barrier over the MT_THREADS
+// threads between the two.
+template <bool WINDOW>
 __device__ __forceinline__ void mt_normal_segment(uint32_t* __restrict__ ring, const int tid,
                                                   const uint32_t* __restrict__ states, const int q,
-                                                  unsigned long long L, unsigned long long offset,
-                                                  unsigned long long n, float* __restrict__ z) {
-  const unsigned long long seg_begin = (unsigned long long)q * L;
-  const unsigned long long lo = max(seg_begin, offset);
-  const unsigned long long hi = min(seg_begin + L, offset + n);
-  if (lo >= hi) return;  // uniform over the MT_THREADS threads
-  // positions relative to the segment start fit 32 bits (L <= 2^30); lo_rel and hi_rel are
-  // multiples of 16, so each 16-group lies wholly inside or wholly outside the window
-  const int lo_rel = (int)(lo - seg_begin), hi_rel = (int)(hi - seg_begin);
-  const int rounds = ((hi_rel + MT_N - 1) / MT_N + MT_ROUND - 1) / MT_ROUND;
+                                                  unsigned long long L, unsigned long long s,
+                                                  unsigned long long n, unsigned long long lo,
+                                                  unsigned long long hi, float* __restrict__ z) {
+  constexpr int RW = MT_ROUND * MT_N;  // stream words per round
+  // positions relative to the segment start fit 32 bits (L <= 2^30).  A main group at relative
+  // position p writes outputs [p + ofs, p + ofs + 16); the tail's outputs [n - 16, n) sit at
+  // relative positions [tail_p - 16, tail_p).  Outputs [lo, hi) are relative [lo_rel, *_hi).
+  const long long ofs = (long long)q * L - (long long)s;
+  const unsigned long long kept = (n & 15) ? n - 16 : n;  // outputs of main groups the tail leaves
+  const int lo_rel = mt_rel((long long)lo - ofs, L);
+  const int main_hi = mt_rel((long long)min(hi, kept) - ofs, L);
+  const int tail_hi = mt_rel((long long)hi - ofs, L);
+  const long long tail_p = (long long)(s + n) - (long long)q * L;
+  const bool tail = WINDOW && (n & 15) && hi > n - 16 && tail_p >= 0 && tail_p < (long long)L;
+  const int main_end = min(main_hi, (int)L);  // main groups of the segment start below it
+  int rounds = (main_end > 0 && main_end + 15 > lo_rel) ? (main_end + RW - 1) / RW : 0;
+  if (tail) rounds = max(rounds, (int)tail_p / RW + 1);
+  if (rounds == 0) return;  // uniform over the MT_THREADS threads
   if (tid < MT_PRODUCERS) {
     constexpr int W = MT_N - MT_M;  // 227
-    // the start window W_{qL} plays block -1
     const uint32_t* w = states + (size_t)q * MT_N;
-    uint32_t* start = ring + (MT_RING - 1) * MT_N;
+    uint32_t* start = mt_block(ring, -1);
     for (int t = tid; t < MT_N; t += MT_PRODUCERS) start[t] = w[t];
     mt_bar_sync<MT_BAR_PROD, MT_PRODUCERS>();
     for (int r = 0; r < rounds; ++r) {
@@ -122,8 +159,8 @@ __device__ __forceinline__ void mt_normal_segment(uint32_t* __restrict__ ring, c
       }
       for (int i = 0; i < MT_ROUND; ++i) {
         const int b = r * MT_ROUND + i;
-        const uint32_t* cur = ring + ((b + MT_RING - 1) % MT_RING) * MT_N;
-        uint32_t* nxt = ring + (b % MT_RING) * MT_N;
+        const uint32_t* cur = mt_block(ring, b - 1);
+        uint32_t* nxt = mt_block(ring, b);
         // wave 0: k in [0,227): x[k], x[k+1], x[k+397] all in the previous block
         if (tid < W) nxt[tid] = mt_twist(cur[tid], cur[tid + 1], cur[tid + MT_M]);
         mt_bar_sync<MT_BAR_PROD, MT_PRODUCERS>();
@@ -135,6 +172,11 @@ __device__ __forceinline__ void mt_normal_segment(uint32_t* __restrict__ ring, c
           const int k = 2 * W + tid;
           const uint32_t c = (k + 1 < MT_N) ? cur[k + 1] : nxt[0];
           nxt[k] = mt_twist(cur[k], c, nxt[k - W]);
+        } else if (WINDOW && i == MT_ROUND - 1 && tid < MT_N - 2 * W + 16) {
+          // after the round's last block: word k < 16 of the next block (wave 0 of that block,
+          // whose inputs nxt[k], nxt[k+1], nxt[k+397] came from waves 0 and 1)
+          const int k = tid - (MT_N - 2 * W);
+          nxt[MT_N + k] = mt_twist(nxt[k], nxt[k + 1], nxt[k + MT_M]);
         }
         mt_bar_sync<MT_BAR_PROD, MT_PRODUCERS>();
       }
@@ -143,32 +185,62 @@ __device__ __forceinline__ void mt_normal_segment(uint32_t* __restrict__ ring, c
     }
   } else {
     const int c = tid - MT_PRODUCERS;
-    const int blk = c / (MT_N / 8), item = c % (MT_N / 8);  // block of the round, item in the block
-    const int word = 16 * (item >> 1) + 4 * (item & 1);      // u[j0] of the item's group
-    const long long seg_to_z = (long long)seg_begin - (long long)offset;  // < 0 only in the first segment
-    // 16-byte stores need z 16-byte aligned (every word offset below is a multiple of 4)
-    const bool vec = ((reinterpret_cast<uintptr_t>(z) & 15) == 0);
+    // the item's group: c < MT_ITEMS: block c / 78 of each round, group (c % 78) / 2 of the block,
+    // every round; c = MT_ITEMS + h: the tail group, once.  In round r it starts at relative
+    // position p = r * RW + at and is the item's iff p lies in [p_min, p_max).  The item's output
+    // j (0..3, 8..11) is at relative position p + j + to_out and is written iff that lies in
+    // [lo_rel, end), i.e. iff p + j lies in [w_lo, w_hi).
+    const int half = 4 * (c & 1);  // j0 of the item (78 items per block: c and item have one parity)
+    int at, p_min, p_max, shift, end;
+    if (c < MT_ITEMS) {
+      at = (c / (MT_N / 8)) * MT_N + (WINDOW ? (int)(s & 15) : 0) + 16 * ((c % (MT_N / 8)) >> 1);
+      p_min = lo_rel - 15;
+      p_max = main_end;
+      shift = 0;
+      end = main_hi;
+    } else {
+      at = (int)tail_p % RW;
+      p_min = (tail && c < MT_ITEMS + 2) ? (int)tail_p : 0;
+      p_max = (tail && c < MT_ITEMS + 2) ? (int)tail_p + 1 : 0;
+      shift = 16;
+      end = tail_hi;
+    }
+    const int to_out = half - shift, w_lo = lo_rel - to_out, w_hi = end - to_out;
+    float* const zq = z + (ofs - (long long)lo + to_out);  // the item's output j of p lands at zq[p + j]
+    // 16-byte ring loads and z stores where the item's words and outputs allow (RW % 4 == 0: the
+    // same in every round)
+    const bool ld128 = !WINDOW || ((at + half) & 3) == 0;
+    const bool st128 = (reinterpret_cast<uintptr_t>(zq + at) & 15) == 0;
     for (int r = 0; r < rounds; ++r) {
       if (r & 1) mt_bar_sync<MT_BAR_FULL + 1, MT_THREADS>();
       else mt_bar_sync<MT_BAR_FULL, MT_THREADS>();
-      const int b = r * MT_ROUND + blk;
-      const int group = b * MT_N + (word & ~15);  // position of the group relative to the segment
-      if (c < MT_ITEMS && group >= lo_rel && group < hi_rel) {
-        const uint32_t* x = ring + (b % MT_RING) * MT_N + word;
-        const uint4 a = *reinterpret_cast<const uint4*>(x);
-        const uint4 s = *reinterpret_cast<const uint4*>(x + 8);
+      const int p = r * RW + at;
+      if (p >= p_min && p < p_max) {
+        const uint32_t* x = ring + (r & 1) * MT_ROUND_WORDS + at + half;
+        uint4 a, b;
+        if (ld128) {
+          a = *reinterpret_cast<const uint4*>(x);
+          b = *reinterpret_cast<const uint4*>(x + 8);
+        } else {
+          a = make_uint4(x[0], x[1], x[2], x[3]);
+          b = make_uint4(x[8], x[9], x[10], x[11]);
+        }
         float4 zc, zs;
-        mt_box_muller(a.x, s.x, zc.x, zs.x);
-        mt_box_muller(a.y, s.y, zc.y, zs.y);
-        mt_box_muller(a.z, s.z, zc.z, zs.z);
-        mt_box_muller(a.w, s.w, zc.w, zs.w);
-        float* zp = z + (seg_to_z + b * MT_N + word);  // >= 0: group >= lo_rel
-        if (vec) {
+        mt_box_muller(a.x, b.x, zc.x, zs.x);
+        mt_box_muller(a.y, b.y, zc.y, zs.y);
+        mt_box_muller(a.z, b.z, zc.z, zs.z);
+        mt_box_muller(a.w, b.w, zc.w, zs.w);
+        float* zp = zq + p;
+        if (!WINDOW || (st128 && p >= w_lo && p + 12 <= w_hi)) {
           *reinterpret_cast<float4*>(zp) = zc;
           *reinterpret_cast<float4*>(zp + 8) = zs;
         } else {
-          zp[0] = zc.x; zp[1] = zc.y; zp[2] = zc.z; zp[3] = zc.w;
-          zp[8] = zs.x; zp[9] = zs.y; zp[10] = zs.z; zp[11] = zs.w;
+          const float v[8] = {zc.x, zc.y, zc.z, zc.w, zs.x, zs.y, zs.z, zs.w};
+#pragma unroll
+          for (int t = 0; t < 8; ++t) {
+            const int j = (t & 3) + (t & 4) * 2;  // j0 + t, then j0 + 8 + t
+            if (p + j >= w_lo && p + j < w_hi) zp[j] = v[t];
+          }
         }
       }
       if (r + 2 < rounds) {  // producers wait on it
@@ -179,10 +251,12 @@ __device__ __forceinline__ void mt_normal_segment(uint32_t* __restrict__ ring, c
   }
 }
 
-// Host side of the replay up to the normal stage (mt19937.cu): checks the window, then seeds
-// and jumps, leaving the start state W_{qL} of every segment q the window [offset, offset+n)
-// touches in `workspace` (tio_randn_mt19937_workspace_bytes).  q_lo, q_hi: those segments.
-int mt_start_states(uint64_t seed, uint64_t offset, uint64_t n, const void* table, void* workspace,
-                    size_t workspace_bytes, cudaStream_t st, const char* who, int* q_lo, int* q_hi);
+// Host side of the replay up to the normal stage (mt19937.cu): seeds and jumps, leaving the
+// start state W_{qL} of every segment q in [q_lo, q_hi) in `workspace`, the segments that hold
+// stream words [first_word, last_word] (the first words of the groups a draw needs).  Checks
+// the table's reach and the workspace size ((q_hi + kS1) states).
+int mt_start_states(uint64_t seed, uint64_t first_word, uint64_t last_word, const void* table,
+                    void* workspace, size_t workspace_bytes, cudaStream_t st, const char* who,
+                    int* q_lo, int* q_hi);
 
 }  // namespace tio

@@ -624,31 +624,35 @@ def intensity_fused(
     big_r: int = 0, axes_mask: int = 0, mean: Tensor | None = None, std: Tensor | None = None,
     keep: Tensor | None = None, z: Tensor | None = None, z2: Tensor | None = None,
     philox_seed: int = 0, noise_mode: int = 0, rician: bool = False,
-    gamma: Tensor | None = None, z_replay: tuple[int, int] | None = None,
+    gamma: Tensor | None = None, z_replay: tuple[int, ...] | None = None,
 ) -> Tensor:
     """Fused bias -> blur -> noise -> gamma (two HBM passes); any stage optional.
 
     Compose-level fusion of consecutive intensity transforms; a single transform
     is a call with only its own stage set.
 
-    ``z_replay`` = (seed, offset) instead of ``z``: the normals are elements
-    [offset, offset + src.numel()) of `randn_mt19937(seed)`.  When the chain has a first pass
-    and a J/K pass of table radius <= 6 on 16-byte aligned rows, the normals are generated
-    inside the first pass (`tio_intensity_pass1_with_normals`) instead of before it; the
-    result is the same bit for bit.
+    ``z_replay`` instead of ``z``: (seed, offset) for the normals of `randn_mt19937(seed, offset,
+    src.numel())`, or (seed, offset, n, lo) for outputs [lo, lo + src.numel()) of the draw of n
+    normals at stream word ``offset`` (a slice of the batch a draw was made for).  When the
+    normals are a draw of their own on 16-word boundaries and the chain has a first pass and a
+    J/K pass of table radius <= 6 on 16-byte aligned rows, they are generated inside the first
+    pass (`tio_intensity_pass1_with_normals`) instead of before it; the result is the same bit
+    for bit.
     """
     src = _batch(src, "intensity_fused")
     b, c, i, j, k = src.shape
     if z_replay is not None:
-        seed, offset = z_replay
+        seed, offset, n, lo = z_replay if len(z_replay) == 4 else (*z_replay, src.numel(), 0)
+        hi = lo + src.numel()
+        aligned = _mt_aligned_draw(offset, n, lo, hi)
         blur_jk = taps is not None and bool(axes_mask & 6) and big_r <= 6
         first_pass = coarse is not None or (taps is not None and bool(axes_mask & 1))
-        if (blur_jk and first_pass and noise_mode == 1 and not rician and k % 4 == 0
-                and src.data_ptr() % 16 == 0 and src.numel() % 16 == 0):
+        if (aligned is not None and blur_jk and first_pass and noise_mode == 1 and not rician
+                and k % 4 == 0 and src.data_ptr() % 16 == 0):
             return _intensity_fused_pass1_normals(
                 src, coarse, bias_identity, bias_divide, taps, radius, big_r, axes_mask, mean, std,
-                keep, gamma, seed, offset)
-        z = randn_mt19937(seed, offset, src.numel(), src.device).view(src.shape)
+                keep, gamma, seed, aligned)
+        z = randn_mt19937(seed, offset, n, src.device, lo=lo, hi=hi).view(src.shape)
     dst = torch.empty_like(src)
     # the J/K pass alone reads src directly; after a first pass it reads the scratch buffer
     two_pass = taps is not None and axes_mask & 6 and (coarse is not None or axes_mask & 1)
@@ -762,21 +766,47 @@ def _mt_table(device: torch.device) -> Tensor:
     return table
 
 
-def randn_mt19937(seed: int, offset: int, n: int, device, out: Tensor | None = None) -> Tensor:
-    """Elements [offset, offset+n) of ``torch.randn(N, generator=CPU mt19937(seed))``
-    computed on ``device`` (to ~1 ulp of the host's libm).  Needs offset, n
-    multiples of 16 and offset + n <= 2**31; callers keep ragged tails on the host."""
+def mt_draw_words(n: int) -> int:
+    """Words of the CPU generator's stream that ``torch.randn(n)`` takes, n >= 16: the n
+    uniforms, then 16 more when n % 16 != 0 (normal_fill recomputes its last 16 outputs)."""
+    return n + (16 if n % 16 else 0)
+
+
+def _mt_aligned_draw(offset: int, n: int, lo: int, hi: int) -> int | None:
+    """Outputs [lo, hi) of the draw of n at ``offset`` are the draw of hi - lo at the returned
+    offset when all four are multiples of 16 (whole 16-groups of an aligned draw); else None."""
+    return offset + lo if offset % 16 == 0 and n % 16 == 0 and lo % 16 == 0 and hi % 16 == 0 else None
+
+
+def randn_mt19937(seed: int, offset: int, n: int, device, out: Tensor | None = None, *,
+                  lo: int = 0, hi: int | None = None) -> Tensor:
+    """Outputs [lo, hi) (default: all n) of ``torch.randn(n, generator=g)`` for a CPU mt19937
+    generator ``g`` seeded with ``seed`` that has already used ``offset`` words of its stream
+    (for an aligned ``offset``: elements [offset, offset+n) of ``torch.randn(N, generator=CPU
+    mt19937(seed))``), computed on ``device`` to ~1 ulp of the host's libm.  Any offset, n >= 16,
+    0 <= lo < hi <= n, and the draw must end within the jump table's reach:
+    offset + `mt_draw_words`(n) <= 2**31."""
     device = torch.device(device)
-    if n < 16 or n % 16 or offset % 16 or offset + n > MT_MAX_WORDS:
-        raise ValueError("randn_mt19937: offset and n must be multiples of 16, n >= 16,"
-                         " offset + n <= 2**31")
-    z = torch.empty(n, dtype=torch.float32, device=device) if out is None else out
+    hi = n if hi is None else hi
+    if n < 16 or offset < 0 or not 0 <= lo < hi <= n:
+        raise ValueError(f"randn_mt19937: needs n >= 16, offset >= 0 and 0 <= lo < hi <= n,"
+                         f" got offset={offset} n={n} lo={lo} hi={hi}")
+    if offset + mt_draw_words(n) > MT_MAX_WORDS:
+        raise ValueError(f"randn_mt19937: the draw of {n} at stream word {offset} ends beyond 2**31")
+    z = torch.empty(hi - lo, dtype=torch.float32, device=device) if out is None else out
     lib = _native.lib()
-    ws_bytes = lib.tio_randn_mt19937_workspace_bytes(offset, n)
-    workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
     table = _mt_table(device)
-    _launch("tio_randn_mt19937", device, int(seed) & 0xFFFFFFFF, offset, n, _ptr(z), _ptr(table),
-            _ptr(workspace), ws_bytes)
+    aligned = _mt_aligned_draw(offset, n, lo, hi)
+    if aligned is not None:
+        ws_bytes = lib.tio_randn_mt19937_workspace_bytes(aligned, hi - lo)
+        workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
+        _launch("tio_randn_mt19937", device, int(seed) & 0xFFFFFFFF, aligned, hi - lo, _ptr(z), _ptr(table),
+                _ptr(workspace), ws_bytes)
+        return z
+    ws_bytes = lib.tio_randn_mt19937_window_workspace_bytes(offset, n)
+    workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
+    _launch("tio_randn_mt19937_window", device, int(seed) & 0xFFFFFFFF, offset, n, lo, hi, _ptr(z),
+            _ptr(table), _ptr(workspace), ws_bytes)
     return z
 
 

@@ -193,7 +193,7 @@ def _noise_mode() -> str:
     """"exact" (default): the normals are the torch.randn draws of the recorded
     CPU-generator seed — the reference's stream (noise.py:166-178) — replayed on
     the device by `ops.randn_mt19937`, or under the first pass of the fused chain
-    (host torch.randn only for ragged shapes).
+    (host torch.randn only for draws below 16 values or beyond the jump table's reach).
     "philox": in-kernel counter-based normals — same distribution, other stream."""
     mode = os.environ.get("TIO_B200_NOISE", "exact").lower()
     if mode not in ("exact", "philox"):
@@ -217,17 +217,17 @@ class Noise(IntensityTransform):
         return True
 
     def supports_chunks(self, batch: SubjectsBatch) -> bool:
-        # the device replay of torch's normal stream starts on 16-word boundaries; the
-        # counter-based stream indexes voxels of the tensor it is given
+        # a slice's normals are a window of the draw over the whole batch, which the device
+        # replay makes for draws of 16 or more values; the counter-based stream indexes voxels of
+        # the tensor it is given
         if _noise_mode() != "exact":
             return False
-        images = self._get_images(batch).values()
+        sizes = [int(np.prod(ib.data.shape)) for ib in self._get_images(batch).values()]
+        if any(n < 16 for n in sizes):
+            return False
         # one stream per application, continued across images and the second Rician draw: all of
         # it must lie inside the jump table's reach, or the one-shot path (host draws) takes over
-        words = sum(int(np.prod(ib.data.shape)) for ib in images) * (2 if self.rician else 1)
-        if words > ops.MT_MAX_WORDS:
-            return False
-        return all(int(np.prod(ib.data.shape[1:])) % 16 == 0 for ib in images)
+        return sum(ops.mt_draw_words(n) for n in sizes) * (2 if self.rician else 1) <= ops.MT_MAX_WORDS
 
     def make_params(self, batch: SubjectsBatch) -> dict[str, Any]:
         seed = int(torch.randint(0, 2**31, (1,)).item())  # drawn first (noise.py:75)
@@ -260,36 +260,37 @@ def _noise_stage_factory(params):
     consumed = [0]  # words of the seed's stream used so far (across images and draws)
 
     def draw(shape, device, defer=False):
-        """Next ``prod(shape)`` normals of the stream: on the device when the
-        position allows (multiples of 16), else with torch.randn on the host,
-        which the generator object keeps aligned with ``consumed``.  ``defer``: a device draw
-        is returned as (seed, start) for `ops.intensity_fused` to make (``z_replay``)."""
+        """Normals of the next draw of the stream for a tensor of ``shape``: the draw of
+        ``prod(shape)`` values, or, while `Compose` streams slices, rows [b0, b1) of the draw over
+        the whole batch (its outputs [per * b0, per * b1)).  On the device for draws of 16 or more
+        values within the jump table's reach, else with torch.randn on the host, which the
+        generator object keeps at ``consumed``.  ``defer``: a device draw is returned as
+        (seed, start, n, lo) for `ops.intensity_fused` to make (``z_replay``)."""
         n = int(np.prod(shape))
         info = chunk_info()
-        if info is None:
-            start, n_full = consumed[0], n
-        else:  # rows [b0, b1) of a draw over the whole batch
-            per = n // shape[0]
-            start, n_full = consumed[0] + per * info.b0, per * info.total
-        on_device = (not ragged[0] and n >= 16 and n % 16 == 0 and start % 16 == 0
-                     and n_full % 16 == 0 and start + n <= ops.MT_MAX_WORDS
+        lo, n_full = (0, n) if info is None else (n // shape[0] * info.b0, n // shape[0] * info.total)
+        start = consumed[0]
+        on_device = (not on_host[0] and n_full >= 16 and start + ops.mt_draw_words(n_full) <= ops.MT_MAX_WORDS
                      and device.type == "cuda")
         if info is not None and not on_device:
-            raise RuntimeError("Noise: this batch cannot be streamed in slices (ragged normal stream)")
-        if n_full < 16 or n_full % 16:
-            ragged[0] = True  # torch's tail/scalar paths: stay on the host from here on
-        consumed[0] += n_full + (16 if (n_full >= 16 and n_full % 16) else 0)
+            raise RuntimeError("Noise: this batch cannot be streamed in slices (host normal stream)")
+        if n_full < 16:
+            on_host[0] = True  # torch's scalar path: its word count is not followed, stay on the host
+        consumed[0] += ops.mt_draw_words(n_full) if n_full >= 16 else n_full
         if on_device:
             if defer:
-                return (params["seed"], start), None
-            return ops.randn_mt19937(params["seed"], start, n, device).view(shape), None
-        # host path: fast-forward the CPU generator to `start` if the device path was used
+                return (params["seed"], start, n_full, lo), None
+            return ops.randn_mt19937(params["seed"], start, n_full, device, lo=lo, hi=lo + n).view(shape), None
+        # host path: fast-forward the CPU generator to `start` past the device draws, each of which
+        # took 16k words or m + 16 >= 33 (a draw of m % 16 != 0): skip is 16k or >= 33
         if host_state[0] != start:
             skip = start - host_state[0]
-            if skip % 16 == 0 and skip >= 16:
+            if skip % 16 == 0:
                 torch.randn(skip, generator=generator)
+            elif skip >= 33:
+                torch.randn(skip - 16, generator=generator)  # ragged: skip - 16 values, 16 more words
             else:
-                raise RuntimeError("Noise: cannot realign the host generator (ragged stream)")
+                raise RuntimeError("Noise: cannot realign the host generator")
         pin = torch.cuda.is_available()
         z = torch.empty(shape, dtype=torch.float32, pin_memory=pin)
         torch.randn(shape, generator=generator, out=z)
@@ -297,7 +298,7 @@ def _noise_stage_factory(params):
         return None, z
 
     host_state = [0]
-    ragged = [False]
+    on_host = [False]
 
     def stage(ib, index):
         shape = ib.data.shape
