@@ -537,6 +537,42 @@ int tio_axis_resample(const void* src, void* dst, int dtype, int B, int C, int I
                       int linear, void* stream);
 
 /*
+ * The adjoints of tio_interpolate and tio_axis_resample for fp32 gradients, one launch each:
+ * grad_in is fully written (no memset), each voxel gathered from grad_out in an order fixed by the
+ * tables, with no atomics, so the result is deterministic.  Every term the forward reads is kept,
+ * zero weights included, so a NaN / Inf in grad_out spreads as in the reference's backward.
+ *
+ * tio_interpolate_backward: grad_in (volumes, I, J, K) from grad_out (volumes, OI, OJ, OK), the
+ * transpose of tio_interpolate with the same tables inverted per axis (tables.py,
+ * interpolate_adjoint_tables).  Replaces ATen's upsample_trilinear3d_backward (align_corners=True)
+ * and upsample_nearest3d_backward, the backward of Resize's F.interpolate and of the two
+ * F.interpolate of _simulate_anisotropy.
+ *   ptr  [(I+1)+(J+1)+(K+1)] int32 device: per axis (I, then J, then K) the CSR row starts of each
+ *        input index, as offsets into ent / wt
+ *   ent  int32 device: output index of each entry; entries of an input index in ascending output
+ *   wt   fp32 device: weight of each entry (nearest: 1)
+ * grad_in = sum over the three windows of ((w_i*w_j)*w_k)*g, I then J then K, each ascending.
+ * volumes*I*J*ceil(K/128) must be below 2^31.
+ *
+ * tio_axis_resample_backward: grad_in (B, C, I, J, K) from grad_out of the same shape, the transpose
+ * of tio_axis_resample with the same axis and w.  Replaces the backward of the gathers and the
+ * four elementwise ops of _simulate_anisotropy_per_instance (torch.gather's scatter_add).
+ *   axis [B] int32 device: as tio_axis_resample (-1: grad_in = grad_out for the element)
+ *   ptr  [B*(L+1)] int32 device: for element b and input plane p along its axis, the row start of p
+ *        in the element's entries
+ *   ent  [B*2L] int32 device: 2*o for output o with lo[o] = p, 2*o + 1 for hi[o] = p, ascending o
+ *   w    [B*L] fp32 device: the forward's weights (NULL when `linear` = 0)
+ * plane p gets the sum of (1 - w[o])*g_o (lo entries, 1 - w rounded as in the forward) and w[o]*g_o
+ * (hi entries); nearest (`linear` = 0) the sum of g_o; planes no output reads get 0.
+ */
+int tio_interpolate_backward(const float* grad_out, float* grad_in, int volumes, int I, int J, int K,
+                             int OI, int OJ, int OK, const int32_t* ptr, const int32_t* ent,
+                             const float* wt, void* stream);
+int tio_axis_resample_backward(const float* grad_out, float* grad_in, int B, int C, int I, int J, int K,
+                               const int32_t* axis, const int32_t* ptr, const int32_t* ent,
+                               const float* w, int L, int linear, void* stream);
+
+/*
  * Clamp, Mask and Swap (intensity/clamp.py, mask.py, swap.py of the reference), one launch each.
  * Image dtypes are tio_dtype codes, TIO_F16 / TIO_BF16 / TIO_F64 included.
  *

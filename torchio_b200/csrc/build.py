@@ -19,7 +19,7 @@ HERE = Path(__file__).resolve().parent
 ROOT = HERE.parent.parent
 SOURCES = ["error.cu", "resample.cu", "resample_tile.cu", "resample_fast.cu", "resample_backward.cu", "upload.cu", "fused_intensity.cu",
            "mt19937_jump.cpp", "mt19937.cu", "patches.cu", "stats.cu", "labels.cu", "labels_to_image.cu",
-           "label_maps.cu", "interpolate.cu", "clamp_mask_swap.cu", "components.cu", "permute.cu", "spike.cu",
+           "label_maps.cu", "interpolate.cu", "interpolate_backward.cu", "clamp_mask_swap.cu", "components.cu", "permute.cu", "spike.cu",
            "ghosting.cu", "motion.cu", "aggregate.cu", "bspline.cu", "pca.cu"]
 HEADERS = [HERE / "common.cuh", HERE / "resample_common.cuh", HERE / "resample_tile.cuh", HERE / "tma.cuh",
            HERE / "mt19937_layout.h", HERE / "mt19937_normal.cuh", HERE / "label_lookup.cuh", HERE / "image_dtype.cuh",

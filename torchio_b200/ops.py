@@ -964,6 +964,42 @@ def axis_resample(src: Tensor, axis: np.ndarray, lo: np.ndarray, hi: np.ndarray,
     return dst
 
 
+def interpolate_backward(grad_out: Tensor, in_shape, ptr: np.ndarray, ent: np.ndarray, wt: np.ndarray) -> Tensor:
+    """The fp32 (B, C, *in_shape) gradient of `interpolate`'s input for the fp32 (B, C, OI, OJ, OK)
+    gradient ``grad_out`` of its output (`tio_interpolate_backward`), from the CSR tables of
+    `tables.resize_adjoint_tables` / `tables.anisotropy_shared_adjoint_tables`.  Deterministic: a
+    gather in a fixed order, no atomics."""
+    grad_out = _batch(grad_out, "interpolate_backward", dtypes=(torch.float32,))
+    b, c, oi, oj, ok = grad_out.shape
+    i, j, k = (int(s) for s in in_shape)
+    grad_in = torch.empty((b, c, i, j, k), dtype=torch.float32, device=grad_out.device)
+    if grad_in.numel():
+        if not grad_out.numel():
+            return grad_in.zero_()
+        ptr_d, ent_d, wt_d = upload(grad_out.device, ptr, ent, wt)
+        _launch("tio_interpolate_backward", grad_out.device, _ptr(grad_out), _ptr(grad_in), b * c, i, j, k,
+                oi, oj, ok, _ptr(ptr_d), _ptr(ent_d), _ptr(wt_d))
+    return grad_in
+
+
+def axis_resample_backward(grad_out: Tensor, axis: np.ndarray, w: np.ndarray, ptr: np.ndarray, ent: np.ndarray, *,
+                           linear: bool) -> Tensor:
+    """The fp32 gradient of `axis_resample`'s input for the fp32 gradient ``grad_out`` of its output
+    (`tio_axis_resample_backward`): ``axis`` and ``w`` as in the forward call, (ptr, ent) from
+    `tables.anisotropy_instance_adjoint_tables`.  Deterministic: a gather in a fixed order."""
+    grad_out = _batch(grad_out, "axis_resample_backward", dtypes=(torch.float32,))
+    b, c, i, j, k = grad_out.shape
+    grad_in = torch.empty_like(grad_out)
+    if grad_out.numel():
+        if linear:
+            axis_d, w_d, ptr_d, ent_d = upload(grad_out.device, axis, w, ptr, ent)
+        else:
+            (axis_d, ptr_d, ent_d), w_d = upload(grad_out.device, axis, ptr, ent), None
+        _launch("tio_axis_resample_backward", grad_out.device, _ptr(grad_out), _ptr(grad_in), b, c, i, j, k,
+                _ptr(axis_d), _ptr(ptr_d), _ptr(ent_d), _ptr(w_d), int(ptr.shape[1]) - 1, int(bool(linear)))
+    return grad_in
+
+
 # ---- Clamp, Mask, Swap (intensity/clamp.py, mask.py, swap.py) ----------------------------------
 
 

@@ -380,14 +380,44 @@ def _pack_axes(axes) -> tuple[np.ndarray, np.ndarray | None]:
     return idx, lam
 
 
+# One axis of a tio_interpolate pass is named by (n_in, n_out, linear, down): ATen's resize of
+# n_in -> n_out, or with ``down`` > 0 Anisotropy's degraded axis (n_in = n_out = L, nearest down to
+# ``down``, back up with the composed up table).  The forward and adjoint tables of each axis are
+# cached per name.
+
+def _resize_axes(in_shape, out_shape, linear: bool) -> list[tuple[int, int, bool, int]]:
+    in_shape, out_shape = tuple(int(s) for s in in_shape), tuple(int(s) for s in out_shape)
+    linear = linear and in_shape != out_shape  # ATen's trilinear copies: identity nearest tables
+    return [(i, o, linear, 0) for i, o in zip(in_shape, out_shape)]
+
+
+def _anisotropy_shared_axes(shape, axis: int, factor: float, linear: bool) -> list[tuple[int, int, bool, int]]:
+    shape = [int(s) for s in shape]
+    length = shape[axis]
+    down = max(1, round(length / factor))
+    linear = linear and down != length  # D == L: ATen's trilinear pass is a copy
+    axes = [(n, n, linear, 0) for n in shape]
+    axes[range(3)[axis]] = (length, length, linear, down)
+    return axes
+
+
+@functools.lru_cache(maxsize=1024)
+def _forward_axis(n_in: int, n_out: int, linear: bool, down: int):
+    """(i0, i1, l0, l1) (linear) or i0 (nearest) of one named axis."""
+    if not down:
+        return aten_linear_axis(n_in, n_out) if linear else aten_nearest_axis(n_in, n_out)
+    down_map = aten_nearest_axis(n_in, down)
+    if linear:
+        i0, i1, l0, l1 = aten_linear_axis(down, n_out)
+        return down_map[i0], down_map[i1], l0, l1
+    return down_map[aten_nearest_axis(down, n_out)]
+
+
 def resize_tables(in_shape, out_shape, linear: bool) -> tuple[np.ndarray, np.ndarray | None]:
     """(idx, lam) of ``F.interpolate(size=out_shape, mode="trilinear", align_corners=True)``
     (``linear``) or ``mode="nearest"`` on CUDA; lam is None for a nearest pass.  ATen's trilinear
     copies when the shapes are equal, which the identity nearest tables reproduce."""
-    in_shape, out_shape = tuple(int(s) for s in in_shape), tuple(int(s) for s in out_shape)
-    if linear and in_shape != out_shape:
-        return _pack_axes([aten_linear_axis(i, o) for i, o in zip(in_shape, out_shape)])
-    return _pack_axes([aten_nearest_axis(i, o) for i, o in zip(in_shape, out_shape)])
+    return _pack_axes([_forward_axis(*a) for a in _resize_axes(in_shape, out_shape, linear)])
 
 
 def anisotropy_shared_tables(shape, axis: int, factor: float, linear: bool):
@@ -397,19 +427,58 @@ def anisotropy_shared_tables(shape, axis: int, factor: float, linear: bool):
     composed with the down map; the other axes keep their size in both passes, so their up tables
     are ATen's L -> L ones (trilinear: weight 1 on the voxel, 0 on its neighbour, both read).
     D == L makes the trilinear pass a copy in ATen."""
-    shape = [int(s) for s in shape]
-    length = shape[axis]
-    down = max(1, round(length / factor))
-    down_map = aten_nearest_axis(length, down)
-    axis = range(3)[axis]
-    if linear and down != length:
-        axes = [aten_linear_axis(n, n) for n in shape]
-        i0, i1, l0, l1 = aten_linear_axis(down, length)
-        axes[axis] = (down_map[i0], down_map[i1], l0, l1)
+    return _pack_axes([_forward_axis(*a) for a in _anisotropy_shared_axes(shape, axis, factor, linear)])
+
+
+# ---- adjoint tables: the forward taps inverted per input index (tio_*_backward) ----------------
+
+
+def invert_taps(src: np.ndarray, out: np.ndarray, n_in: int) -> tuple[np.ndarray, np.ndarray]:
+    """CSR inverse of a list of taps: tap t reads input ``src[t]`` for output ``out[t]``.  Returns
+    (ptr [n_in + 1], order) with ``order`` the tap numbers sorted stably by (input, output): the
+    taps of input x are order[ptr[x]:ptr[x + 1]], in ascending output, and two taps of one output
+    on one input (the pair that collapses onto the last plane) in the order they are listed.  No
+    monotonicity of ``src`` is assumed.  Every tap is kept, zero weights included."""
+    src = np.asarray(src, dtype=np.int64)
+    order = np.lexsort((np.asarray(out, dtype=np.int64), src))
+    ptr = np.zeros(n_in + 1, dtype=np.int64)
+    np.cumsum(np.bincount(src, minlength=n_in), out=ptr[1:])
+    return ptr, order
+
+
+@functools.lru_cache(maxsize=1024)
+def _adjoint_axis(n_in: int, n_out: int, linear: bool, down: int):
+    """(ptr [n_in + 1], output index, weight) of one named axis: the taps of input x, lower taps
+    listed before upper ones, are entries ptr[x]:ptr[x + 1]."""
+    taps = _forward_axis(n_in, n_out, linear, down)
+    o = np.arange(n_out, dtype=np.int64)
+    if linear:
+        src, out, w = np.concatenate(taps[:2]), np.concatenate([o, o]), np.concatenate(taps[2:])
     else:
-        axes = [aten_nearest_axis(n, n) for n in shape]
-        axes[axis] = down_map[aten_nearest_axis(down, length)]
-    return _pack_axes(axes)
+        src, out, w = taps, o, np.ones(n_out, dtype=np.float32)
+    ptr, order = invert_taps(src, out, n_in)
+    return ptr, out[order], w[order].astype(np.float32)
+
+
+def _pack_adjoint(axes) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """[(ptr, out, w) per axis] -> the (ptr, ent, wt) tables of tio_interpolate_backward: one entry
+    list for the three axes, each axis's row starts offset into it."""
+    ptrs, base = [], 0
+    for ptr, out, _ in axes:
+        ptrs.append(ptr + base)
+        base += len(out)
+    return (np.concatenate(ptrs).astype(np.int32), np.concatenate([a[1] for a in axes]).astype(np.int32),
+            np.concatenate([a[2] for a in axes]).astype(np.float32))
+
+
+def resize_adjoint_tables(in_shape, out_shape, linear: bool) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """(ptr, ent, wt) of the transpose of the `resize_tables` pass (tio_interpolate_backward)."""
+    return _pack_adjoint([_adjoint_axis(*a) for a in _resize_axes(in_shape, out_shape, linear)])
+
+
+def anisotropy_shared_adjoint_tables(shape, axis: int, factor: float, linear: bool):
+    """(ptr, ent, wt) of the transpose of the `anisotropy_shared_tables` pass."""
+    return _pack_adjoint([_adjoint_axis(*a) for a in _anisotropy_shared_axes(shape, axis, factor, linear)])
 
 
 @functools.lru_cache(maxsize=1024)
@@ -461,3 +530,36 @@ def anisotropy_instance_tables(shape, axes, factors, linear: bool):
         axis[b] = a
         lo[b, :length], hi[b, :length], w[b, :length] = rows
     return axis, lo, hi, w
+
+
+@functools.lru_cache(maxsize=1024)
+def _instance_adjoint_axis(length: int, down: int, linear: bool) -> tuple[np.ndarray, np.ndarray]:
+    """(ptr [length + 1], entries) of one element's axis: the entries of input plane p are
+    2*o (lo[o] = p) and 2*o + 1 (hi[o] = p, linear only), ascending o, lo before hi."""
+    lo, hi, _ = _instance_axis(length, down, linear)
+    o = np.arange(length, dtype=np.int64)
+    if linear:
+        src, code = np.concatenate([lo, hi]), np.concatenate([2 * o, 2 * o + 1])
+    else:
+        src, code = lo, 2 * o
+    ptr, order = invert_taps(src, code, length)
+    return ptr, code[order]
+
+
+def anisotropy_instance_adjoint_tables(shape, axes, factors, linear: bool) -> tuple[np.ndarray, np.ndarray]:
+    """(ptr [B, L + 1], ent [B, 2L]) int32 of tio_axis_resample_backward for the
+    `anisotropy_instance_tables` of the same arguments, L = max(shape).  An element with axis -1
+    has empty rows; past the axis's length, rows repeat the last start (empty)."""
+    shape = [int(s) for s in shape]
+    width = max(shape)
+    n = len(axes)
+    ptr = np.zeros((n, width + 1), dtype=np.int32)
+    ent = np.zeros((n, 2 * width), dtype=np.int32)
+    for b, (a, f) in enumerate(zip(axes, factors)):
+        if not f > 1.0:
+            continue
+        length = shape[a]
+        p, e = _instance_adjoint_axis(length, anisotropy_down_size(length, f), linear)
+        ptr[b, :length + 1], ptr[b, length + 1:] = p, p[-1]
+        ent[b, :len(e)] = e
+    return ptr, ent

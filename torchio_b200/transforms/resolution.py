@@ -10,15 +10,21 @@ to its dtype as the reference's ``data.float()`` ... ``.to(dtype)`` do:
   (Anisotropy's nearest-down map composed into the up table, so the downsampled tensor never exists);
 - Anisotropy's per-instance path: `ops.axis_resample` from `tables.anisotropy_instance_tables`, which
   restate that path's own int64 / fp32 index arithmetic (it picks different planes than ATen's).
+
+With `set_differentiable(True)`, a scalar image that requires grad goes through the same calls as
+graph nodes (`autograd.interpolate`, `autograd.axis_resample`), whose backwards are the transposes of
+these tables (`tables.*_adjoint_tables`), gathered in a fixed order; a label map that requires grad
+is refused.
 """
 
 from __future__ import annotations
 
+import functools
 from typing import Any
 
 import torch
 
-from .. import ops, tables
+from .. import autograd, ops, tables
 from ..data import LabelMap, SubjectsBatch
 from ..params import to_nonneg_range
 from .base import SpatialTransform, Transform
@@ -71,20 +77,39 @@ class Anisotropy(Transform):
         self._tag_batched(params, batch, n, keep, ["axis", "factor"])
         return params
 
+    differentiable = True  # scalar images: autograd.interpolate / autograd.axis_resample
+
     def apply_transform(self, batch: SubjectsBatch, params: dict[str, Any]) -> SubjectsBatch:
         per_instance = self._is_per_instance_params(params)
-        for _, ib in batch.images.items():
-            linear = not issubclass(ib._image_class, LabelMap) and self.image_interpolation != "nearest"
+        for name, ib in batch.images.items():
+            is_label = issubclass(ib._image_class, LabelMap)
+            linear = not is_label and self.image_interpolation != "nearest"
+            graph, data = _graph_input("Anisotropy", name, ib.data, is_label)
             if per_instance:
-                ib.data = _degrade_per_instance(ib.data, params["axis"], params["factor"], linear)
+                ib.data = _degrade_per_instance(data, params["axis"], params["factor"], linear, graph)
             elif params["factor"] > 1.0:
-                idx, lam = tables.anisotropy_shared_tables(ib.data.shape[2:], params["axis"], params["factor"],
-                                                           linear)
-                ib.data = ops.interpolate(ib.data, ib.data.shape[2:], idx, lam)
+                args = (data.shape[2:], params["axis"], params["factor"], linear)
+                idx, lam = tables.anisotropy_shared_tables(*args)
+                if graph:
+                    ib.data = autograd.interpolate(data, data.shape[2:], idx, lam,
+                                                   functools.partial(tables.anisotropy_shared_adjoint_tables, *args))
+                else:
+                    ib.data = ops.interpolate(data, data.shape[2:], idx, lam)
         return batch
 
 
-def _degrade_per_instance(data, axes: list[int], factors: list[float], linear: bool):
+def _graph_input(transform: str, name: str, data, is_label: bool):
+    """(records a graph node, the tensor to pass on) for image ``name``: a label map that requires
+    grad is refused, and with grad mode off an image that requires grad runs the usual kernels."""
+    graph = autograd.records_graph(data)
+    if graph and is_label:
+        autograd.refuse(transform, f'label map "{name}"')
+    if not graph and data.requires_grad and ops.differentiable_default():
+        data = data.detach()
+    return graph, data
+
+
+def _degrade_per_instance(data, axes: list[int], factors: list[float], linear: bool, graph: bool = False):
     """_simulate_anisotropy_per_instance (anisotropy.py:132-177): untouched when no element has a
     factor > 1, an error for an active axis outside {0, 1, 2}."""
     active = [f > 1.0 for f in factors]
@@ -93,6 +118,9 @@ def _degrade_per_instance(data, axes: list[int], factors: list[float], linear: b
     if any(a < 0 or a > 2 for a, on in zip(axes, active) if on):
         raise ValueError(f"Anisotropy axis must be in {{0, 1, 2}}, got {sorted(set(axes))}")
     axis, lo, hi, w = tables.anisotropy_instance_tables(data.shape[2:], axes, factors, linear)
+    if graph:
+        adjoint = functools.partial(tables.anisotropy_instance_adjoint_tables, data.shape[2:], axes, factors, linear)
+        return autograd.axis_resample(data, axis, lo, hi, w, adjoint, linear=linear)
     return ops.axis_resample(data, axis, lo, hi, w, linear=linear)
 
 
@@ -113,17 +141,24 @@ class Resize(SpatialTransform):
         self.image_interpolation = image_interpolation
         self.label_interpolation = label_interpolation
 
+    differentiable = True  # scalar images: autograd.interpolate
+
     def make_params(self, batch: SubjectsBatch) -> dict[str, Any]:
         return {"target_shape": self.target_shape}
 
     def apply_transform(self, batch: SubjectsBatch, params: dict[str, Any]) -> SubjectsBatch:
         target = [int(s) for s in params["target_shape"]]
-        for _, ib in batch.images.items():
+        for name, ib in batch.images.items():
             is_label = issubclass(ib._image_class, LabelMap)
             mode = self.label_interpolation if is_label else self.image_interpolation
-            old_shape = tuple(ib.data.shape[2:])
+            graph, data = _graph_input("Resize", name, ib.data, is_label)
+            old_shape = tuple(data.shape[2:])
             idx, lam = tables.resize_tables(old_shape, target, mode != "nearest")
-            ib.data = ops.interpolate(ib.data, target, idx, lam)
+            if graph:
+                adjoint = functools.partial(tables.resize_adjoint_tables, old_shape, target, mode != "nearest")
+                ib.data = autograd.interpolate(data, target, idx, lam, adjoint)
+            else:
+                ib.data = ops.interpolate(data, target, idx, lam)
             for index, affine in enumerate(ib.affines):
                 matrix = affine.numpy().copy()
                 for axis in range(3):
